@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py -- frames/s of the dense tracking-and-fusion hot path on B200 (BASELINE.json metric).
+"""bench.py -- frames/s of the dense tracking-and-fusion hot path on one H100 (BASELINE.json metric).
 
 Workload (N=1): BASELINE.json configs[1] -- synthetic 640x480 RGB-D stream into a 512^3 TSDF volume (6 m), ICP-only
 tracker {10,5,4} iterations, volume shifting on (-t 14, overlap 2).  A "step" is ONE frame through
@@ -11,11 +11,14 @@ integrate -> raycast + model pyramid.
           inside the timed region (kt_process_frame).
   roofline / stages : CUDA-event stage timers of the tracker (on its own stream), algorithmic bytes from DESIGN.md section 4.
   cpu_baseline : the CPU oracle ("port") on a bounded sample of the same workload, on this box's host cores.
-  --impl reference : the reference's OWN CUDA kernels (oracle/_ref/libkt_ref_512.so, compiled from /root/reference with
-          two mechanical patches), driven by the restated host loop with the reference's launch / sync pattern.
+  --impl reference : the reference's OWN CUDA kernels (oracle/_ref/libkt_ref_512.so, compiled from the reference sources by
+          oracle/build_ref.sh with two mechanical patches), driven by the restated host loop with the reference's launch / sync pattern.
           The reference has no CPU implementation of this path; if the library is missing, the CPU oracle port is timed.
 Timing: W>=3 warm-up frames, exactly K timed frames between barrier + cuda synchronize, max over ranks, CUDA clocks sampled
-with nvidia-smi during the timed region.  Inputs: 96 distinct frames (147 MB) cycled, i.e. larger than the 126 MB L2.
+with nvidia-smi during the timed region.  Inputs: 96 distinct frames (147 MB) cycled, i.e. larger than the 50 MB L2.
+--dump-outputs DIR: after the timed frames, what the last timed frame returned to its caller (R, t, global_t, voxel_wrap of
+kt_process_frame_device) and the surface it predicted for the next frame (model vertex / normal maps of level 0 with invalid pixels
+zeroed, and their validity masks) as DIR/<name>.npy, float32 / float64, all finite.  The inputs are seeded, so two builds run with the same arguments can be compared output for output.
 Multi-GPU (torchrun): the headline line is weak scaling -- rank r tracks its own stream into its own volume (independent sessions, no
 data-path collective).  At every N the same JSON line carries a `zslab` sub-record: ONE stream fused into ONE 1024^3 volume shared by all
 N GPUs (BASELINE configs[3]; replicated TSDF with owner P2P stores, block-cyclic colour planes, banded ray cast with the model-map
@@ -153,7 +156,7 @@ def measured_peak():
             return float(json.load(open(p))["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
         except Exception:
             pass
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, "NVIDIA H100 SXM data sheet (HBM3), not measured"
 
 
 def dist_setup(n_gpus, init=True):
@@ -213,7 +216,7 @@ def shared_volume_leg(kb, torch, args, world, rank, local, device, dev_depth, de
     if world > 1:
         from kintinuous_b200 import mgpu
         mgpu.connect(trk)
-    steps = max(20, min(args.steps, 100))
+    steps = args.steps
     prewarm = 40
 
     def run(k, i):
@@ -264,7 +267,7 @@ def run_reference(args, world, rank, local):
     from oracle import refbind
     import kintinuous_b200 as kb
     cfg = kb.Config.default(rows=ROWS, cols=COLS, vol=args.vol, odometry=args.odometry)
-    n_frames = N_INPUT_FRAMES                         # the same frame set as the b200 arm (same_config)
+    n_frames = N_INPUT_FRAMES                         # the same frame set as the product arm (same_config)
     frames = make_stream(n_frames)
     PREWARM = int(os.environ.get("KT_BENCH_PREWARM", "150"))
     warmup = max(3, args.warmup)
@@ -286,7 +289,7 @@ def run_reference(args, world, rank, local):
         t = ref.tracker(refbind.TrackerConfig.from_kt(cfg))
         sync = torch.cuda.synchronize
         kind, cores = "reference", 1
-        sample = "every step: the reference's own CUDA kernels (oracle/_ref/libkt_ref_<vol>.so = /root/reference src/frontend/cuda/*.cu recompiled for sm_100) on cuda:0, original launch shapes and 26 syncs/frame, restated host loop on 1 host thread, blocking H2D from pageable memory"
+        sample = "every step: the reference's own CUDA kernels (oracle/_ref/libkt_ref_<vol>.so = the reference's src/frontend/cuda/*.cu recompiled for sm_90) on cuda:0, original launch shapes and 26 syncs/frame, restated host loop on 1 host thread, blocking H2D from pageable memory"
     else:
         o = refbind.CpuOracle()
         cores = o.lib.ktoracle_hardware_threads() or 1
@@ -295,11 +298,11 @@ def run_reference(args, world, rank, local):
         sync = lambda: None
         kind = "port"
         sample = f"oracle/_ref unavailable: CPU oracle port on {cores} threads"
-        args.steps = min(args.steps, 8); warmup = 1; PREWARM = 0
-        line["steps"], line["warmup"] = args.steps, warmup
+        warmup = 1; PREWARM = 0
+        line["warmup"] = warmup
         line["config"]["prewarm_frames"] = 0; line["config"]["untimed_frames_before_region"] = 2
     i = 0
-    for _ in range(PREWARM + warmup + 1):             # the same untimed lead-in as the b200 arm (GPU clocks, allocator, first shifts)
+    for _ in range(PREWARM + warmup + 1):             # the same untimed lead-in as the product arm (GPU clocks, allocator, first shifts)
         d, c = frames[pingpong(i, n_frames)]; t.process(d, c, i); i += 1
     sync(); t0 = time.perf_counter()
     for _ in range(args.steps):
@@ -310,6 +313,25 @@ def run_reference(args, world, rank, local):
                  "cpu_baseline": {"value": v, "unit": "frames/s", "cores": int(cores), "kind": kind, "sample": sample},
                  "e2e": {"value": v, "unit": "frames/s", "h2d_bytes_per_step": 0, "d2h_bytes_per_step": 0}})
     print(json.dumps(line), flush=True)
+
+
+def dump_outputs(out_dir, trk, pose):
+    """The last timed frame's results: its pose as kt_process_frame_device returned it, and the model maps it ray cast for the next frame.
+    A map marks a pixel without surface by NaN in its x plane and leaves the other planes as the buffer held them, so each map is written
+    as a validity mask (1 / 0) and the map with every plane of an invalid pixel set to 0: all values finite, nothing stale compared."""
+    os.makedirs(out_dir, exist_ok=True)
+    R, t, g, w = pose.as_tuple()
+    arrays = {"R": R, "t": t, "global_t": g, "voxel_wrap": w.astype(np.float64)}
+    for name, which in (("model_vmap", 2), ("model_nmap", 3)):
+        m = trk.download_map(which, 0)
+        valid = ~np.isnan(m[0])
+        m[:, ~valid] = 0.0
+        arrays[name] = m
+        arrays[name + "_valid"] = valid.astype(np.float32)
+    for name, a in arrays.items():
+        if not np.isfinite(a).all():
+            raise RuntimeError(f"--dump-outputs: {name} has non-finite values")
+        np.save(os.path.join(out_dir, f"{name}.npy"), np.ascontiguousarray(a))
 
 
 def main():
@@ -328,7 +350,10 @@ def main():
     ap.add_argument("--vol", type=int, default=VOL)
     ap.add_argument("--scale", type=int, default=1, help="image scale: 1 = 640x480 (configs 1-3), 2 = 1280x960 (configs[4])")
     ap.add_argument("--odometry", type=int, default=0, help="0 ICP (configs[1]), 2 ICP+RGB-D (configs[2])")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write what the last timed frame computed to DIR/<name>.npy")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
     global ROWS, COLS, P_LEVELS, N_INPUT_FRAMES
     if args.scale != 1:
         ROWS, COLS = 480 * args.scale, 640 * args.scale
@@ -370,16 +395,17 @@ def main():
 
     def run(tracker, use_host, steps, start):
         i = start
+        run.last = None
         for _ in range(steps):
             j = pingpong(i, n)
             jn = pingpong(i + 1, n)
             # kt_prefetch_frame (public API hint): the next frame's copy and pose-independent front end overlap this frame's fusion
             if use_host:
-                tracker.process_frame(pin_depth[j].data_ptr(), pin_rgb[j].data_ptr(), i)
+                run.last = tracker.process_frame(pin_depth[j].data_ptr(), pin_rgb[j].data_ptr(), i)
                 if not args.no_prefetch:
                     tracker.prefetch_frame(pin_depth[jn].data_ptr(), pin_rgb[jn].data_ptr())
             else:
-                tracker.process_frame_device(dev_depth[j], dev_rgb[j], i)
+                run.last = tracker.process_frame_device(dev_depth[j], dev_rgb[j], i)
                 if not args.no_prefetch:
                     tracker.prefetch_frame(dev_depth[jn], dev_rgb[jn])
             i += 1
@@ -416,6 +442,8 @@ def main():
             raise RuntimeError("device stopwatch failed")
         dt = max_over_ranks(dt, world, device)
         results[leg] = {"dt": dt, "wall": max_over_ranks(wall, world, device), "launches": l1 - l0}
+        if leg == "device" and args.dump_outputs and rank == 0:
+            dump_outputs(args.dump_outputs, trk, run.last)
         if leg == "device":
             # stage timers (CUDA events on the tracker's stream) over a few extra frames, outside the timed region
             trk.set_stage_timing(True)
@@ -467,29 +495,13 @@ def main():
     # DESIGN.md section 4); duration from CUDA events recorded around that launch on the tracker's stream
     icp_ms = results.get("icp_kernel_ms", 0.0) or st[1]
     ach = icp_bytes / (icp_ms * 1e-3) / 1e9 if icp_ms > 0 else None
-    traffic = None
-    traffic_file = None
-    try:                                                      # dram__bytes_read.sum + dram__bytes_write.sum of the committed ncu capture
-        import csv, glob
-        kname = "icp_frame_kernel" if args.odometry == 0 else "rgbd_frame_kernel"
-        cands = sorted(glob.glob(os.path.join(ROOT, "profiles", f"r2_ncu_full_*{kname}*.csv"))) or sorted(glob.glob(os.path.join(ROOT, "profiles", f"r1_ncu_full_v10_{kname}.csv")))
-        traffic_file = os.path.relpath(cands[-1], ROOT)
-        rows = list(csv.reader(open(cands[-1])))
-        H, U, Vv = rows[0], rows[1], rows[2]
-        def val(name):
-            i = H.index(name); x = float(Vv[i]); u = U[i].lower()
-            return x * (1e6 if u.startswith("mbyte") else 1e3 if u.startswith("kbyte") else 1e9 if u.startswith("gbyte") else 1.0)
-        traffic = val("dram__bytes_read.sum") + val("dram__bytes_write.sum")
-    except Exception:
-        traffic = None
     # compulsory DRAM bytes of the launch: the four map sets of the levels in use, read once (48 B/pixel; later iterations hit L2 / smem)
     compulsory = sum(per_px * P_LEVELS[l] for l in range(4) if ICP_ITERS[l] > 0)
     roofline = {"kernel": kernel_name, "bound": "hbm",
-                "achieved": ach, "peak": peak, "unit": "GB/s", "frac": (ach / peak) if ach else None, "traffic": traffic,
-                "traffic_source": f"ncu --set full capture {traffic_file} (dram__bytes_read.sum + dram__bytes_write.sum, one launch); not re-measured in this run" if traffic else None,
+                "achieved": ach, "peak": peak, "unit": "GB/s", "frac": (ach / peak) if ach else None,
                 "compulsory_dram_bytes": compulsory, "frac_compulsory_dram": (compulsory / (icp_ms * 1e-3) / 1e9 / peak) if icp_ms > 0 else None,
                 "peak_source": peak_src, "bytes_per_launch": icp_bytes, "avg_launch_ms": icp_ms,
-                "note": "algorithmic bytes / CUDA-event time of that launch; the kernel is latency-bound by design at 640x480 (19 sequential reduce+solve steps, each a grid-wide exchange; inputs L2- / shared-memory-resident so DRAM traffic equals one compulsory read of the maps, far below the algorithmic bytes); see DESIGN.md section 4 and profiles/r2_ncu_summary.md",
+                "note": "algorithmic bytes / CUDA-event time of that launch; the kernel is latency-bound by design at 640x480 (19 sequential reduce+solve steps, each a grid-wide exchange; inputs L2- / shared-memory-resident so DRAM traffic equals one compulsory read of the maps, far below the algorithmic bytes); see DESIGN.md section 4",
                 "dominant_stage": dom}
     dt = results["device"]["dt"]
     streams = 1 if zslab else world          # z-slab: all ranks work on ONE stream (strong scaling)

@@ -1,5 +1,5 @@
 /*
- * kintinuous_b200 -- C ABI of the B200-native dense tracking-and-fusion hot path.
+ * kintinuous_b200 -- C ABI of the H100-native dense tracking-and-fusion hot path.
  *
  * This header is the drop-in boundary (SURVEY.md section 8b): plain pointers and sizes, no torch /
  * Eigen / OpenCV / PCL types.  Each entry point names the reference interface it replaces
@@ -91,7 +91,7 @@ typedef struct kt_point_xyzrgbnormal {
 typedef struct kt_ctx kt_ctx;
 
 KT_API const char* kt_last_error(void);
-/* 1 when the library was built with the sm_100a kernels and a CUDA device is usable. */
+/* 1 when the library was built with the sm_90a kernels and a CUDA device is usable. */
 KT_API int kt_cuda_available(void);
 
 /* ---- tracker: replaces class KintinuousTracker (KintinuousTracker.h:85-172) ---- */

@@ -1,4 +1,4 @@
-// kintinuous_b200 -- shared device/host helpers for the sm_100a kernels.
+// kintinuous_b200 -- shared device/host helpers for the sm_90a kernels.
 //
 // Numerics contract: every kernel in csrc/ is compiled with the reference's own nvcc numerics
 // flags (--ftz=true --prec-div=false --prec-sqrt=false, reference CMakeLists.txt:47) and keeps the

@@ -7,7 +7,7 @@
 // NEIGHBOUR's colour with r/b swapped and this voxel's weight as alpha (Q8), and is shifted by
 // realVoxelWrap*cell - size/2 (:310-312).  The +z neighbour is not range-checked: at z = V-1 it wraps to logical
 // plane 0 through the cyclic addressing (Q12).  Point order is unspecified in the reference too (global atomicAdd).
-// B200 design: the box is walked in STORAGE-contiguous order (x fastest) by a grid sized to the SM count, compaction
+// Design: the box is walked in STORAGE-contiguous order (x fastest) by a grid sized to the SM count, compaction
 // is a warp-level prefix (shuffles + one atomicAdd per warp), points are written as two 16-byte stores, and -- unlike
 // the reference (extract.cu:268-288) -- nothing is ever written past the caller's capacity.
 // Bound: HBM, 6 B per slab voxel + 32 B per point.
@@ -165,7 +165,7 @@ int extract_slice(const int16_t* tsdf, const float3& volume_size, int vol, void*
     p.out = (uint4*)out; p.capacity = (unsigned int)capacity; p.counter = counter_dev;
     size_t total = (size_t)(maxX - minX) * (maxY - minY) * (maxZ - minZ);
     size_t blocks = (total + 255) / 256;
-    int grid = (int)(blocks < (size_t)148 * 16 ? blocks : (size_t)148 * 16);
+    int grid = (int)(blocks < (size_t)device_info().sm_count * 16 ? blocks : (size_t)device_info().sm_count * 16);
     extract_kernel<<<grid, 256, 0, s>>>(p);
     KT_LAUNCH_CHECK();
     return 0;
@@ -184,7 +184,7 @@ int extract_slice_mg(const VolumeView& vv, const float3& volume_size, int vol, v
     p.vv = vv; p.multi = 1;
     size_t total = (size_t)(maxX - minX) * (maxY - minY) * (maxZ - minZ);
     size_t blocks = (total + 255) / 256;
-    int grid = (int)(blocks < (size_t)148 * 16 ? blocks : (size_t)148 * 16);
+    int grid = (int)(blocks < (size_t)device_info().sm_count * 16 ? blocks : (size_t)device_info().sm_count * 16);
     extract_kernel<<<grid, 256, 0, s>>>(p);
     KT_LAUNCH_CHECK();
     return 0;

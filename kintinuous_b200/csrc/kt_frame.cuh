@@ -6,7 +6,7 @@
 
 namespace kt {
 
-enum { FRAME_THREADS = 512, STAGE_MAX_K = 17 };   // 17 passes x 6 planes x 2 KB = 204 KB of shared memory: 1280x960 level 0 still fits
+enum { FRAME_THREADS = 512, STAGE_MAX_K = 18 };   // 18 passes x 6 planes x 2 KB = 216 KB: the most an H100 block's 227 KB take beside the static smem
 
 __device__ __forceinline__ void grid_barrier(unsigned int* bar, unsigned int target)
 {
@@ -29,7 +29,7 @@ __device__ __forceinline__ void grid_barrier(unsigned int* bar, unsigned int tar
 // matters to the solve (DESIGN.md section 3.2).  Latency: one atomic to L2 plus one poll round trip after the LAST CTA arrived
 // (measured with tools/tail_bench.cu against the counter barrier + partial re-read it replaces).
 // Requirements: gridDim.x <= 255; the words are zero when the launch starts (the host keeps them so, kt_tracker.cu).
-enum { XW_STRIDE = 160, XW_WORDS = 2 * 32 * XW_STRIDE };     // 1280 B apart: measured best of 8 / 256 / 1280 / 2304 / 4352 / 16640 B (tools/tail_bench.cu)
+enum { XW_STRIDE = 160, XW_WORDS = 2 * 32 * XW_STRIDE };     // 1280 B apart (tools/tail_bench.cu times other strides)
 
 __device__ __forceinline__ void red_add_u64(unsigned long long* p, unsigned long long v)
 { asm volatile("red.relaxed.gpu.global.add.u64 [%0], %1;" :: "l"(p), "l"(v) : "memory"); }

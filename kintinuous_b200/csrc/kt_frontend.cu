@@ -8,13 +8,13 @@
 //             computeDerivativeImages: shortDepthToMetres, imageBGRToIntensity, pyrDownGaussF x3, pyrDownUcharGauss x3, the 3x3
 //             gradient at all four levels (bilateral_pyrdown.cu:172-331, RGBDOdometry.cpp:140-175)
 //
-// B200 design.  A CTA owns a 64 x 32 pixel tile of level 0 and produces ITS part of every output of every pyramid level from shared
+// Design:  A CTA owns a 64 x 32 pixel tile of level 0 and produces ITS part of every output of every pyramid level from shared
 // memory: the tile is staged once with the halo the three 5x5 decimations need (level l computes its owned pixels plus a halo of
 // HL_l / HR_l pixels, HL_l = 2 HL_{l+1} + 2, HR_l = 2 HR_{l+1} + 1: 14 / 15 pixels at level 0 for the depth pyramid, 22 / 15 with the
 // photometric pyramids whose gradient needs one more left neighbour at level 3).  The halo is recomputed by the neighbouring CTAs --
 // 2.4x redundant work on the cheap 25-tap decimations (the 169-tap bilateral filter is NOT recomputed: it is launch 1) -- which buys
 // independence: no level ever goes back to HBM before the next one reads it, the vertex map is never re-read to make normals, and
-// 150 CTAs (one wave of the 148 SMs) replace 11-23 dependent launches of <= 76 800 threads.  Per-pixel arithmetic is the
+// 150 CTAs (about one wave on 132 SMs) replace 11-23 dependent launches of <= 76 800 threads.  Per-pixel arithmetic is the
 // reference's, expression by expression (window clipping Q1, integer weight count Q2, stale y/z planes Q7, the gradient's tap walk),
 // with the contractions its build has (read off the SASS: fma(g, .587, fma(r, .114, b * .299)), fma(v, w, sum)) written out.
 // Bound: HBM streaming of the outputs (51 B per level-0 pixel ICP-only, 74 B with the photometric set), latency of three

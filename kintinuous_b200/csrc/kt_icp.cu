@@ -6,9 +6,9 @@
 //   struct JtJJtrSE3 (29 floats)                                         cuda/internal.h:98-149
 //   the host half of ICPOdometry::getIncrementalTransformation           ICPOdometry.cpp:86-180
 //
-// B200 design (DESIGN.md section 3.2): the reference launches 64 CTAs x 128 threads (8 192 threads on a 148-SM part), a second
+// Design (DESIGN.md section 3.2): the reference launches 64 CTAs x 128 threads (8 192 threads on a 132-SM part), a second
 // 1-CTA kernel, then cudaDeviceSynchronize + 116-byte D2H + host LDLT, 19x per frame.  Two kernels here:
-//   icp_frame_kernel  the tracker's path: ONE persistent cooperative launch per FRAME (148 CTAs x 512 threads, one per SM) runs all
+//   icp_frame_kernel  the tracker's path: ONE persistent cooperative launch per FRAME (132 CTAs x 512 threads, one per SM) runs all
 //                     levels and iterations; the CTA's contiguous slice of the current maps is staged in shared memory by TMA bulk
 //                     copies once per level; per iteration: batched model-map gathers, warp transpose-reduce, one 128-byte partial
 //                     per CTA, ONE grid barrier, then every CTA sums the partials in the same fixed order and solves the 6x6
@@ -142,12 +142,12 @@ icp_kernel(const IcpParams p)
 //            the current vertex stay in registers between the two halves); 29 sums per thread;
 //   reduce   warp transpose-sum (lane l ends with component l) -> shared memory -> warp 0 adds the 16 warps in a fixed order;
 //   exchange warp 0: ONE fire-and-forget 64-bit atomic per component into self-counting fixed-point words, poll until all CTAs are
-//            in (grid_sum_words, kt_frame.cuh): no grid barrier, no fence, no re-read of 148 partials;
+//            in (grid_sum_words, kt_frame.cuh): no grid barrier, no fence, no re-read of 132 partials;
 //   solve    lane 0 of warp 0 of EVERY CTA: the same FP64 LDL^T + Rodrigues + pose composition on the same bit-identical totals
 //            (kt_solve.cuh, latency-trimmed form), so no pose broadcast is needed and all CTAs hold identical poses.
 // Two __syncthreads per iteration.  The totals are exact integer sums => deterministic run to run.
 // ICP_BATCH = pixels per thread whose model-map gathers are in flight together (template parameter: 4, or 5 when the level-0 share of a
-// thread is 4 passes + a remainder -- 640x480 on 148 SMs: 4.05 pixels per thread -- so that the remainder does not cost a second batch's
+// thread is 4 passes + a remainder -- 640x480 on 132 SMs: 4.55 pixels per thread -- so that the remainder does not cost a second batch's
 // worth of L2 latency per iteration; the sums are accumulated in pass order either way, so the result does not depend on it)
 
 struct IcpFrameParams {
@@ -159,7 +159,8 @@ struct IcpFrameParams {
     float* trace;
     int* timeout;              // set to 1 if a peer CTA never arrived (bounded poll)
     long long* prof;           // optional: clock64() stamps per iteration from CTA 0 (debug)
-    int stage_k;               // passes of FRAME_THREADS pixels per CTA that fit the shared-memory stage (0 = no staging)
+    int stage_k;               // passes of FRAME_THREADS pixels per CTA held in the shared-memory stage (0 = no staging); a level with
+                               // more passes stages its first stage_k and reads the rest from global memory
     float* host_pose; unsigned int host_seq;      // optional mapped host record: pose (12), time-out (1), sequence number (1)
     PeerWords pw; int rank;                       // pw.world > 1: the pixel rows are split over the ranks of a shared volume (grid_sum_words_mg)
 };
@@ -218,14 +219,15 @@ icp_frame_kernel(const IcpFrameParams p)
         const int i_begin = min(N, gci * q), cnt = min(N, i_begin + q) - i_begin;
         const int n_pass = (q + FRAME_THREADS - 1) / FRAME_THREADS;
         const int ps = p.stage_k * FRAME_THREADS;                    // floats per staged plane
-        const bool staged = (p.stage_k > 0) && (n_pass <= p.stage_k) && ((N & 3) == 0);
+        const bool staged = (p.stage_k > 0) && ((N & 3) == 0);
+        const int n_st = staged ? min(n_pass, p.stage_k) : 0;       // passes read from shared memory; passes n_st.. come from global memory
         if (staged) {
-            // The current vertex / normal maps do not change during the level's iterations: ONE bulk copy per plane (<= 16 KB,
-            // 16-byte aligned) brings the CTA's range into shared memory through the TMA engine; every iteration then reads its
-            // 24 streamed bytes per pixel from shared memory instead of L2.
+            // The current vertex / normal maps do not change during the level's iterations: ONE bulk copy per plane (16-byte aligned)
+            // brings the CTA's range -- its first n_st passes when the range is larger than the stage -- into shared memory through the
+            // TMA engine; every iteration then reads its 24 streamed bytes per pixel from shared memory instead of L2.
             __syncthreads();                                         // previous level's readers are done with the stage
             if (tid == 0) {
-                const unsigned int bytes = (unsigned int)cnt * 4u;
+                const unsigned int bytes = (unsigned int)min(cnt, n_st * FRAME_THREADS) * 4u;
                 mbar_expect_tx(&s_mbar, bytes * 6u);                 // 0 completes the phase for CTAs without pixels at this level
                 if (bytes) {
 #pragma unroll
@@ -255,8 +257,11 @@ icp_frame_kernel(const IcpFrameParams p)
                     for (int b = 0; b < ICP_BATCH; ++b) {
                         const int o = (k0 + b) * FRAME_THREADS + tid;
                         j[b] = -1;
-                        if (k0 + b < n_pass && o < cnt)
-                            j[b] = icp_pixel_project2(make_float3(s_stage[o], s_stage[ps + o], s_stage[2 * ps + o]), cols, rows, intr, Rcurr, tcurr, Rprev_inv, tprev, vg[b], vcp[b]);
+                        if (k0 + b < n_pass && o < cnt) {
+                            const float3 vc = k0 + b < n_st ? make_float3(s_stage[o], s_stage[ps + o], s_stage[2 * ps + o])
+                                                            : make_float3(__ldg(&vmap_curr[i_begin + o]), __ldg(&vmap_curr[i_begin + o + N]), __ldg(&vmap_curr[i_begin + o + 2 * N]));
+                            j[b] = icp_pixel_project2(vc, cols, rows, intr, Rcurr, tcurr, Rprev_inv, tprev, vg[b], vcp[b]);
+                        }
                     }
 #pragma unroll
                     for (int b = 0; b < ICP_BATCH; ++b) {
@@ -268,7 +273,9 @@ icp_frame_kernel(const IcpFrameParams p)
                     for (int b = 0; b < ICP_BATCH; ++b) {
                         if (j[b] >= 0) {
                             const int o = (k0 + b) * FRAME_THREADS + tid;
-                            icp_pixel_finish2(vg[b], vcp[b], make_float3(s_stage[3 * ps + o], s_stage[4 * ps + o], s_stage[5 * ps + o]),
+                            const float3 nc = k0 + b < n_st ? make_float3(s_stage[3 * ps + o], s_stage[4 * ps + o], s_stage[5 * ps + o])
+                                                            : make_float3(__ldg(&nmap_curr[i_begin + o]), __ldg(&nmap_curr[i_begin + o + N]), __ldg(&nmap_curr[i_begin + o + 2 * N]));
+                            icp_pixel_finish2(vg[b], vcp[b], nc,
                                               make_float3(g[b][0], g[b][1], g[b][2]), make_float3(g[b][3], g[b][4], g[b][5]),
                                               Rcurr, Rprev_inv, tprev, dist_thres, angle_thres, sum);
                         }
@@ -415,9 +422,18 @@ int icp_frame(const IcpLevelArgs* levels, const int* iters, const float* pose12_
         }
         di.configured |= 1u;
     }
-    const size_t stage_bytes = (size_t)6 * need_k * FRAME_THREADS * sizeof(float);
-    const bool can_stage = need_k > 0 && need_k <= STAGE_MAX_K && smem_optin > 0 && stage_bytes <= (size_t)(smem_optin - 4096);
-    p.stage_k = can_stage ? need_k : 0;
+    // the stage holds as many passes as the largest level needs, up to what a block's shared memory takes (STAGE_MAX_K on an H100);
+    // a level that needs more stages that many and streams the rest (1280x960 level 0 on 132 SMs: 18 of 19 passes)
+    int stage_k = need_k < STAGE_MAX_K ? need_k : STAGE_MAX_K;
+    const int smem_k = smem_optin > 4096 ? (smem_optin - 4096) / (6 * FRAME_THREADS * (int)sizeof(float)) : 0;
+    if (stage_k > smem_k) stage_k = smem_k;
+    static int stage_knob = -1;                     // KT_ICP_STAGE_PASSES (test hook): a smaller stage, so that 640x480 takes the partial path
+    if (stage_knob < 0) { const char* e = getenv("KT_ICP_STAGE_PASSES"); stage_knob = e ? atoi(e) : 0; }
+    if (stage_knob > 0 && stage_k > stage_knob) stage_k = stage_knob;
+    if (stage_k < 0) stage_k = 0;
+    const size_t stage_bytes = (size_t)6 * stage_k * FRAME_THREADS * sizeof(float);
+    const bool can_stage = stage_k > 0;
+    p.stage_k = stage_k;
     static int batch_knob = -1;                     // KT_ICP_BATCH = 4 | 5 (A/B); default: 5 when the largest level leaves a remainder pass after groups of 4
     if (batch_knob < 0) { const char* e = getenv("KT_ICP_BATCH"); batch_knob = e ? atoi(e) : 0; }
     const int batch = batch_knob == 4 || batch_knob == 5 ? batch_knob : ((need_k % 4 == 1) ? 5 : 4);

@@ -6,7 +6,7 @@
 //   KintinuousTracker::outputPose                                           KintinuousTracker.cpp:199-218 (called per frame, :911-914)
 // outputPose writes  "<utime / 1e6, fixed, 6 decimals> gx gy gz qx qy qz qw\n"  with the floats in the stream's default format (%g,
 // 6 significant digits) and the quaternion from Eigen::Quaternionf(Rcurr).  Eigen is a third-party dependency that is not under
-// /root/reference: its matrix -> quaternion conversion (Eigen/src/Geometry/Quaternion.h, quaternionbase_assign_impl<Other,3,3>, the
+// the reference checkout: its matrix -> quaternion conversion (Eigen/src/Geometry/Quaternion.h, quaternionbase_assign_impl<Other,3,3>, the
 // same in every 3.x release) is restated below in float.  The reference re-opens, appends and closes the file on EVERY frame
 // (SURVEY.md Q14); here the file stays open for the life of the context and every line is flushed.
 #pragma once

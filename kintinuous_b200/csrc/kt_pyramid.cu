@@ -1,4 +1,4 @@
-// kintinuous_b200 -- depth pyramid and vertex / normal maps (sm_100a).
+// kintinuous_b200 -- depth pyramid and vertex / normal maps (sm_90a).
 //
 // Replaces (reference file:line, src/frontend/cuda/):
 //   bilateralFilter / bilateralKernel      bilateral_pyrdown.cu:60-99, :333-343
@@ -7,7 +7,7 @@
 //   createNMap / computeNmapKernel         maps.cu:83-121, :140-155
 //   tranformMaps / tranformMapsKernel      maps.cu:157-222
 //   resizeVMap/NMap / resizeMapKernel      maps.cu:225-308
-// B200 design: the bilateral filter stages a (4+12)x(32+12) depth tile (as float) in shared memory once per
+// Design: the bilateral filter stages a (4+12)x(32+12) depth tile (as float) in shared memory once per
 // CTA (169 taps/pixel come from smem, not L1); vertex and normal maps of ALL pyramid levels are
 // produced by ONE launch straight from the depth pyramid (the vertex map is never re-read to make
 // normals); per-pixel arithmetic keeps the reference's expression order (see kt_common.cuh).
@@ -23,8 +23,8 @@ namespace {
 const float SIGMA_COLOR = 30.f;      // mm   (bilateral_pyrdown.cu:56)
 const float SIGMA_SPACE = 4.5f;      // px   (bilateral_pyrdown.cu:57)
 
-// 32x4-pixel CTAs: at 640x480 the image is 1.35 % more than one full wave of 2048 threads x 148 SMs, so with 512-thread CTAs the
-// last 8 of 600 ran alone after everyone else (ncu: SMs active 66 % of the kernel); 128-thread CTAs make that tail one small CTA long.
+// 32x4-pixel CTAs: 640x480 is not a whole number of waves of 2048 threads per SM, and with 512-thread CTAs the last few of 600 run
+// alone after everyone else; 128-thread CTAs make that tail one small CTA long.
 enum { BIL_TX = 32, BIL_TY = 4, BIL_R = 6, BIL_W = BIL_TX + 2 * BIL_R, BIL_H = BIL_TY + 2 * BIL_R };
 
 // One pixel's 13x13 window from the float tile, taps in the reference's order (rows, then columns).  PRED: window clipped to

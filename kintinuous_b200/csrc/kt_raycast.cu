@@ -4,7 +4,7 @@
 // Replaces (reference, src/frontend/cuda/):
 //   raycast / RayCaster / rayCastKernel          ray_caster.cu:56-471
 //   resizeVMap / resizeNMap (x3 levels)          maps.cu:225-308  (KintinuousTracker.cpp:892-899)
-// B200 design: one CTA = a 16x8 pixel tile; after the march the tile's vertices / normals sit in shared
+// Design: one CTA = a 16x8 pixel tile; after the march the tile's vertices / normals sit in shared
 // memory and the 2x2 means of levels 1..3 (8x4, 4x2, 2x1 pixels per tile) are produced by the same CTA,
 // which removes 6 launches + 6 cudaDeviceSynchronize per frame and the 12 MB re-read of the level-0 maps.
 // Per-ray arithmetic (march step, trilinear taps, gradient normal) keeps the reference's expression
@@ -403,7 +403,7 @@ int raycast(const RaycastArgs& a, cudaStream_t s)
         }
     }
     else if (pow2 && idx32) {
-        // 8 speculative steps per batch at 8 CTAs/SM; measured and dropped: 4 steps per batch (72.3 vs 68.2 us), 10 CTAs/SM (73.2 us, spills)
+        // 8 speculative steps per batch at 8 CTAs/SM (4 steps per batch and 10 CTAs/SM, which spills, were slower)
         raycast_kernel<true, unsigned int, 8, 8, false><<<grid, block, 0, s>>>(p);
     }
     else if (pow2) raycast_kernel<true, size_t, 8, 8, false><<<grid, block, 0, s>>>(p);

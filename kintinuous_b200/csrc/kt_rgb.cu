@@ -11,7 +11,7 @@
 //   computeRgbResidual / RGBResidual / residualKernel   cuda/reduce.cu:668-864
 //   rgbStep / RGBReduction / rgbKernel                  cuda/reduce.cu:423-607
 //   host half of RGBDOdometry::getIncrementalTransformation   RGBDOdometry.cpp:205-370
-// B200 design: no per-call cudaMalloc/cudaFree (the reference allocates the 25-tap table and the reduce
+// Design: no per-call cudaMalloc/cudaFree (the reference allocates the 25-tap table and the reduce
 // scratch on every call, SURVEY.md section 3.2); the warp (K R K^-1, K t) of each iteration is rebuilt on the
 // device from the running estimate; the sigma of the robust weight and the Gauss-Newton solve live in the
 // reduction tails, so an iteration is 2 launches (3 with ICP) and no host round trip.  The tracker itself uses rgbd_frame_kernel:
@@ -613,7 +613,7 @@ int rgbd_frame(const IcpLevelArgs* icp_levels, const RgbLevelArgs* rgb_levels, c
     p.st = state; p.xwords = xwords_dev; p.trace = trace; p.timeout = timeout_dev; p.with_icp = with_icp;
     DeviceInfo& di = device_info();
     const int sms = di.sm_count, smem_optin = di.smem_optin;
-    int grid = sms > 0 ? sms : 148;
+    int grid = sms > 0 ? sms : 132;
     if (grid > 255) grid = 255;                  // the exchange words count arrivals in 8 bits
     int need_k = 0;
     for (int l = 0; l < LEVELS; ++l)

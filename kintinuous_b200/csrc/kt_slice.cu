@@ -5,7 +5,7 @@
 //   pcl::VoxelGrid<PointXYZRGB>, leaf = voxel edge (one centroid per leaf)   :126-148     PCL 1.7.2 filters/impl/voxel_grid.hpp
 //   pcl::NormalEstimation, KdTree, setKSearch(20), viewpoint (0,0,0)         :150-160     PCL 1.7.2 features/normal_3d.h, common/impl/{centroid,eigen}.hpp
 //   pcl::concatenateFields -> PointXYZRGBNormal                              :162
-// PCL is a third-party dependency that is not under /root/reference; its published 1.7.2 algorithms are restated on the CPU by the test
+// PCL is a third-party dependency that is not under the reference checkout; its published 1.7.2 algorithms are restated on the CPU by the test
 // suite's checker (tests/test_slice_oracle.py pins it) and re-designed here:
 //   * no sort, no kd-tree: the leaf grid itself is the spatial index.  A BIT PER LEAF (dx*dy*dz bits, 0.6 MB for a 17-plane slab of a
 //     512^3 volume) marks occupied leaves; a prefix sum of the words' popcounts turns (word, bit) into the output slot, which is

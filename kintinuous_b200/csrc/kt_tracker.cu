@@ -5,7 +5,7 @@
 // TsdfVolume (TSDFVolume.cpp:60-172), ColorVolume, and the drivers ICPOdometry::getIncrementalTransformation
 // (ICPOdometry.cpp:68-186) / RGBDOdometry::getIncrementalTransformation (RGBDOdometry.cpp:165-393).
 //
-// B200 design (DESIGN.md section 3): everything of a frame is enqueued on ONE stream with exactly one host
+// Design (DESIGN.md section 3): everything of a frame is enqueued on ONE stream with exactly one host
 // synchronisation -- after the odometry, because the shift decision and the slice hand-off are host logic in
 // the reference too.  The reference's frame has 59 launches, 26 cudaDeviceSynchronize and 19 blocking D2H
 // copies; here: 6 front-end launches (bilateral, 3 pyrDown, maps, colour prep), ONE cooperative odometry launch (all levels and
@@ -53,7 +53,7 @@ DeviceInfo& device_info()
         DeviceInfo d; d.sm_count = 0; d.smem_optin = 0; d.configured = 0;
         cudaDeviceGetAttribute(&d.sm_count, cudaDevAttrMultiProcessorCount, dev);
         cudaDeviceGetAttribute(&d.smem_optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev);
-        if (d.sm_count <= 0) d.sm_count = 148;
+        if (d.sm_count <= 0) d.sm_count = 132;
         info[dev] = d;
         ready[dev].store(1, std::memory_order_release);
     }

@@ -9,7 +9,7 @@
 // kt_volume_export_reference_layout is a plain copy: tsdf short[V^3] (value * 32767, round toward zero)
 // and colour uchar4[V^3] = {r, g, b, weight}; x fastest; cyclic ("shifting") addressing
 //   storage(x,y,z) = ((x+wx)%V) + ((y+wy)%V)*V + ((z+wz)%V)*V^2        (tsdf_volume.cu:612)
-// B200 re-layout of the WORK, not of the bytes: threads are mapped to STORAGE coordinates (the
+// Re-layout of the WORK, not of the bytes: threads are mapped to STORAGE coordinates (the
 // reference maps them to logical coordinates, so after a shift every warp straddles sector
 // boundaries); a warp always owns one aligned 64-B tsdf segment + one aligned 128-B colour line per z,
 // the z axis is split into 16 chunks (grid.z) for 16x more CTAs than the reference's 1 024, whole columns
@@ -82,7 +82,7 @@ clear_planes_x_kernel(int16_t* __restrict__ tsdf, uchar4* __restrict__ color, in
 // (0 + 0.5f) * cell - t_z and 0 and grow by ONE float addition of cell per z step).  Prologue of the integration, one small launch: entry
 // z is brought there by thread z with the exact fast-forward of kt_replay.cuh (round 1: one thread adding 2 V times, 6 us on the critical
 // path between the odometry and the integration; building the entries inside integrate_kernel -- per thread, or per CTA in shared
-// memory -- was measured and is slower: 66 -> 77 .. 85 us at 512^3), and the other job of this launch is the reset of the odometry
+// memory -- was slower in the design's measurements), and the other job of this launch is the reset of the odometry
 // kernels' exchange words for the next frame (grid_sum_words, kt_frame.cuh): it sits between two odometry launches anyway.
 __global__ void __launch_bounds__(256) ztable_kernel(float* __restrict__ table, int V, float cell_z, float t_z, unsigned long long* __restrict__ reset_words, int reset_count, int reset_stride, int seq)
 {
@@ -368,7 +368,7 @@ integrate_kernel(const IntegrateParams p)
 int fill_zero(void* p, size_t bytes, cudaStream_t s)
 {
     size_t n16 = bytes / 16;
-    int grid = (int)((n16 + 255) / 256 < 148 * 16 ? (n16 + 255) / 256 : 148 * 16);
+    int grid = (int)((n16 + 255) / 256 < (size_t)device_info().sm_count * 16 ? (n16 + 255) / 256 : (size_t)device_info().sm_count * 16);
     if (grid < 1) grid = 1;
     fill_zero_u4<<<grid, 256, 0, s>>>((uint4*)p, n16);
     KT_LAUNCH_CHECK();
@@ -425,11 +425,11 @@ int clear_volume_shared(int axis, int back, const VolumeView& vv, int vol, int c
     int16_t* tsdf = vv.tsdf[vv.rank]; uint8_t* color = vv.color[vv.rank];
     if (axis == 0) {
         size_t total = (size_t)count * V * V;
-        int grid = (int)((total + 255) / 256 < 148 * 16 ? (total + 255) / 256 : 148 * 16);
+        int grid = (int)((total + 255) / 256 < (size_t)device_info().sm_count * 16 ? (total + 255) / 256 : (size_t)device_info().sm_count * 16);
         clear_planes_x_kernel<<<grid, 256, 0, s>>>(tsdf, (uchar4*)color, V, p0, count, vv);
     } else {
         size_t total = (size_t)count * V * (V / 8);
-        int grid = (int)((total + 255) / 256 < 148 * 16 ? (total + 255) / 256 : 148 * 16);
+        int grid = (int)((total + 255) / 256 < (size_t)device_info().sm_count * 16 ? (total + 255) / 256 : (size_t)device_info().sm_count * 16);
         clear_planes_yz_kernel<<<grid, 256, 0, s>>>(tsdf, color, V, axis, p0, count, vv);
     }
     KT_LAUNCH_CHECK();
@@ -464,9 +464,8 @@ int integrate(const IntegrateArgs& a, float* ztable_dev, cudaStream_t s)
     const bool prep = prep_knob != 0 && a.cw && a.rgbf;      // the caller ran color_prep() on this frame's normal map and image
     p.cw = a.cw; p.rgbf = a.rgbf;
     p.ztable = ztable_dev; p.zchunk = V >= 64 ? (V + n_chunks - 1) / n_chunks : V;
-    // z chunks: a warp walks its columns' voxels serially, so a chunk's length is the scheduling quantum of the launch.  Measured on
-    // B200 (640x480 into 512^3, tools/stage_ab.py): 8 chunks 100 us, 16 chunks 78 us, 32 chunks 96 us (per-chunk column setup);
-    // dispatching the far chunks first was slower at every chunk count (89-109 us).
+    // z chunks: a warp walks its columns' voxels serially, so a chunk's length is the scheduling quantum of the launch; 16 chunks
+    // balance that quantum against the per-chunk column setup (KT_INT_ZCHUNKS and tools/stage_ab.py re-measure it).
     p.z_far_first = (a.Rinv.r2.z > 0.f) == (order != 0) ? 1 : 0;          // z component of the camera's viewing axis in the volume frame
     const bool multi = a.multi && a.vv.world > 1;
     p.vv = multi ? a.vv : single_volume(a.tsdf, a.color, V);
@@ -498,9 +497,8 @@ int integrate(const IntegrateArgs& a, float* ztable_dev, cudaStream_t s)
         if (idx32) { if (prep) integrate_kernel<unsigned int, 1, 6, true, true><<<grid, block, 0, s>>>(p); else integrate_kernel<unsigned int, 1, 6, false, true><<<grid, block, 0, s>>>(p); }
         else { if (prep) integrate_kernel<size_t, 1, 6, true, true><<<grid, block, 0, s>>>(p); else integrate_kernel<size_t, 1, 6, false, true><<<grid, block, 0, s>>>(p); }
     } else if (idx32) {
-        // batch depth / CTAs per SM (KT_INT_ZU = 1 or 2 overrides).  Measured (tools/stage_ab.py, 640x480): 512^3 2-voxel batches at 4
-        // CTAs/SM 78 us vs 81 us for 1-voxel steps at 6 CTAs/SM; 1024^3 395 vs 351 us: once the updated region outgrows L2, occupancy
-        // wins.  Also measured and dropped: 3- and 4-voxel batches (82 / 93 us), 2-voxel batches at 5 or 6 CTAs/SM (81 / 91 us, spills)
+        // batch depth / CTAs per SM (KT_INT_ZU = 1 or 2 overrides): 2-voxel batches at 4 CTAs/SM while the updated region stays in L2,
+        // 1-voxel steps at 6 CTAs/SM from 1024^3, where occupancy hides the HBM latency (tools/stage_ab.py compares them).
         const int variant = zu ? zu : (V >= 1024 ? 1 : 2);
         if (prep && (variant == 1 || variant == 2)) {
             if (variant == 1) integrate_kernel<unsigned int, 1, 6, true><<<grid, block, 0, s>>>(p);

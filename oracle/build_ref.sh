@@ -1,13 +1,13 @@
 #!/bin/bash
 # TEST INFRASTRUCTURE ONLY. Builds oracle/_ref/libkt_ref_<VOL>.so: the reference's own CUDA operators
-# (/root/reference/src/frontend/cuda/*.cu + containers/*.cpp, compiled from where they lie) plus
+# ($KT_REFERENCE_ROOT/src/frontend/cuda/*.cu + containers/*.cpp, compiled from where they lie) plus
 # oracle/ref_harness.cu. The reference sources are copied to a TEMPORARY directory only because two files
-# need mechanical patches to compile for sm_100 (SURVEY.md D7) and VOL must become a -D macro (D5):
+# need mechanical patches to compile for sm_90 (SURVEY.md D7) and VOL must become a -D macro (D5):
 #   reduce.cu : __shfl_down(x, offset)  -> __shfl_down_sync(0xffffffff, x, offset)
 #   extract.cu: __all(..)/__ballot(..)  -> *_sync(0xffffffff, ..)
 #   internal.h: #define VOL 512         -> #ifndef VOL / #define VOL 512 / #endif
 # Nothing but the .so lands in the repo tree (oracle/_ref/ is git-ignored). Flags are the reference's own
-# (CMakeLists.txt:47): --ftz=true --prec-div=false --prec-sqrt=false, arch retargeted to sm_100.
+# (CMakeLists.txt:47): --ftz=true --prec-div=false --prec-sqrt=false, arch retargeted to sm_90.
 # usage: oracle/build_ref.sh [VOL ...]   (default: 256 512)
 set -euo pipefail
 REF=${KT_REFERENCE_ROOT:-/root/reference}
@@ -23,7 +23,7 @@ sed -i -E 's/__shfl_down\(([^,]+), offset\)/__shfl_down_sync(0xffffffffu, \1, of
 sed -i -E 's/__all \(/__all_sync (0xffffffffu, /g; s/__ballot \(/__ballot_sync (0xffffffffu, /g' "$TMP/cuda/extract.cu"
 sed -i 's/^#define VOL 512/#ifndef VOL\n#define VOL 512\n#endif/' "$TMP/cuda/internal.h"
 NVCC=${NVCC:-/usr/local/cuda/bin/nvcc}
-FLAGS="-std=c++14 -O3 -gencode arch=compute_100,code=sm_100 --ftz=true --prec-div=false --prec-sqrt=false -Xcompiler -fPIC -w"
+FLAGS="-std=c++14 -O3 -gencode arch=compute_90,code=sm_90 --ftz=true --prec-div=false --prec-sqrt=false -Xcompiler -fPIC -w"
 for V in $VOLS; do
   B=$TMP/build_$V; mkdir -p $B
   pids=()

@@ -6,7 +6,7 @@
 // Two backends instantiate it:
 //   * oracle/kt_oracle_cpu.cpp  -- CPU restatement of every kernel ("port" oracle)
 //   * oracle/ref_harness.cu     -- the reference's own, unmodified CUDA operators compiled from
-//                                  /root/reference (oracle/_ref/libkt_ref_<VOL>.so, "reference" oracle)
+//                                  the reference checkout (oracle/_ref/libkt_ref_<VOL>.so, "reference" oracle)
 // so both run the *same* host logic; the reference host classes themselves cannot be compiled
 // here (they need Eigen/OpenCV/PCL/Boost, none installed -- SURVEY.md D6).
 //

@@ -6,7 +6,7 @@
 //     2. pcl::VoxelGrid     leaf = max voxel edge, one centroid per occupied leaf                        :126-148
 //     3. pcl::NormalEstimation, KdTree, setKSearch(20)                                                   :150-160
 //     4. pcl::concatenateFields -> PointXYZRGBNormal                                                     :162
-// Steps 2 and 3 live in a third-party dependency that is NOT under /root/reference: PCL, "find_package(PCL 1.7)" (src/CMakeLists.txt:52),
+// Steps 2 and 3 live in a third-party dependency that is NOT under the reference checkout: PCL, "find_package(PCL 1.7)" (src/CMakeLists.txt:52),
 // installed by build.sh from the 14.04 PPA = PCL 1.7.2.  This file restates the published algorithms of PCL 1.7.2:
 //     filters/include/pcl/filters/impl/voxel_grid.hpp        VoxelGrid<PointT>::applyFilter
 //     common/include/pcl/common/impl/centroid.hpp            computeMeanAndCovarianceMatrix (single pass, float accumulators)

@@ -2,7 +2,7 @@
 // product path (kintinuous_b200/).
 //
 // C-ABI harness around the reference's OWN CUDA operators (src/frontend/cuda/internal.h:299-536),
-// compiled by oracle/build_ref.sh from the sources where they lie under /root/reference (two
+// compiled by oracle/build_ref.sh from the sources where they lie under the reference checkout (two
 // mechanical sed patches for post-Volta warp intrinsics on a temporary copy, VOL made a -D macro;
 // SURVEY.md D5/D7). Output: oracle/_ref/libkt_ref_<VOL>.so (git-ignored, travels to the GPU box).
 // Nothing from the reference is copied into this repository; this file only CALLS the reference API.

@@ -1,7 +1,7 @@
 """TEST INFRASTRUCTURE ONLY (oracle/): ctypes bindings of the two oracles.
 
   * RefCuda  -- oracle/_ref/libkt_ref_<VOL>.so: the reference's OWN CUDA operators (compiled by
-                oracle/build_ref.sh from /root/reference) behind oracle/ref_harness.cu.  Needs a GPU.
+                oracle/build_ref.sh from the reference checkout) behind oracle/ref_harness.cu.  Needs a GPU.
   * CpuOracle -- oracle/libkt_oracle_cpu.so: the CPU restatement (oracle/kt_oracle_cpu.cpp).
 
 Only tests/, __graft_entry__.smoke() and bench.py's cpu_baseline / --impl reference legs import this.
@@ -127,7 +127,7 @@ class RefCuda:
     def __init__(self, vol: int):
         p = os.path.join(_HERE, "_ref", f"libkt_ref_{vol}.so")
         if not os.path.exists(p):
-            raise FileNotFoundError(f"{p}: run oracle/build_ref.sh {vol} where /root/reference exists")
+            raise FileNotFoundError(f"{p}: run oracle/build_ref.sh {vol} where the reference checkout exists")
         self.lib = C.CDLL(p)
         self.lib.ktref_extract.restype = C.c_size_t
         self.vol = self.lib.ktref_vol()

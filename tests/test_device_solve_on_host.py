@@ -4,6 +4,7 @@ Its source compiles for the host as well (tests/cpp/solve_host.cu), so it is che
 pinned oracle restatements -- including the cases Eigen's pivoted LDLT treats specially (rank-deficient normal matrices)."""
 import ctypes as C
 import os
+import shutil
 import subprocess
 
 import numpy as np
@@ -24,8 +25,9 @@ def solve_lib():
     src = os.path.join(ROOT, "tests", "cpp", "solve_host.cu")
     hdr = os.path.join(ROOT, "kintinuous_b200", "csrc", "kt_solve.cuh")
     if not os.path.exists(so) or os.path.getmtime(so) < max(os.path.getmtime(src), os.path.getmtime(hdr)):
-        subprocess.check_call(["nvcc", "-std=c++17", "-shared", "-Xcompiler", "-fPIC", "-I", os.path.join(ROOT, "kintinuous_b200", "csrc"),
-                               "-gencode", "arch=compute_100a,code=sm_100a", "-o", so, src])
+        nvcc = os.environ.get("NVCC") or shutil.which("nvcc") or "/usr/local/cuda/bin/nvcc"          # the Makefile's default too
+        subprocess.check_call([nvcc, "-std=c++17", "-shared", "-Xcompiler", "-fPIC", "-I", os.path.join(ROOT, "kintinuous_b200", "csrc"),
+                               "-gencode", "arch=compute_90a,code=sm_90a", "-o", so, src])
     return C.CDLL(so)
 
 

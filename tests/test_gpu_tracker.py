@@ -64,43 +64,42 @@ def test_tracker_vs_golden_reference_cuda(built, frames, name, kw, nframes):
 
 
 def test_tracker_vs_reference_cuda_live(built, frames):
-    """Both trackers run here, frame by frame, on the same input (needs oracle/_ref on the box)."""
+    """Frame by frame against the reference tracker's run on the same input (tests/golden/ref_tracker_live_256.npz: its poses, a seeded
+    sample of 50 000 of its touched voxels, its model maps' invalid-pixel masks and a sample of their valid pixels)."""
     import kintinuous_b200 as kb
-    from oracle import refbind
-    if not refbind.RefCuda.available(256):
-        pytest.skip("oracle/_ref not present")
+    g = np.load(os.path.join(GOLDEN, "ref_tracker_live_256.npz"))
     cfg = kb.Config.default(vol=256)
     mine = kb.Tracker(cfg)
-    rt = refbind.RefCuda(256).tracker(refbind.TrackerConfig.from_kt(cfg))
     for k, (d, c) in enumerate(frames):
-        p = mine.process_frame(d, c, k); rt.process(d, c, k)
-        Ra, ta, ga, wa = p.as_tuple(); Rb, tb, gb, wb = rt.pose()
+        p = mine.process_frame(d, c, k)
+        Ra, ta, ga, wa = p.as_tuple(); Rb, tb, wb = g["poses"][k][:9].reshape(3, 3), g["poses"][k][9:12], g["wraps"][k]
         assert np.abs(ta - tb).max() <= 1e-4 and rot_angle(Ra, Rb) <= 1e-4 and (wa == wb).all()
-    ta, ca = mine.export_volume(); tb, cb = rt.export_volume()
-    touched = cb[..., 3] != 0
-    d = np.abs(ta.astype(np.int32) - tb.astype(np.int32))[touched]
-    assert (d <= 1).mean() >= 0.995, float((d <= 1).mean())      # measured 0.9997 (tools/ab_report.py); poses differ by ~1e-6
-    assert (ca[..., 3][touched] == cb[..., 3][touched]).mean() >= 0.999
+    ta, ca = mine.export_volume()
+    idx = g["vol_idx"]
+    d = np.abs(ta.reshape(-1)[idx].astype(np.int32) - g["vol_tsdf"].astype(np.int32))
+    assert (d <= 1).mean() >= 0.995, float((d <= 1).mean())      # poses differ by ~1e-6
+    assert (ca[..., 3].reshape(-1)[idx] == g["vol_weight"]).mean() >= 0.999
     # model maps handed to the next frame (raycast + in-kernel pyramid vs raycast + 6 resize launches)
     for lvl in range(3):
-        va = mine.download_map(2, lvl); vb = rt.download_map(2, lvl)
-        na, nb = np.isnan(va[0]), np.isnan(vb[0])
+        va = mine.download_map(2, lvl)
+        na = np.isnan(va[0]).reshape(-1)
+        nb = np.unpackbits(g[f"map_nan_{lvl}"], count=na.size).astype(bool)
         assert (na != nb).mean() < 2e-3
-        ok = ~na & ~nb
-        assert np.quantile(np.abs(va[:, ok] - vb[:, ok]).max(0), 0.999) < 1e-3
-    mine.close(); rt.close()
+        px = g[f"map_px_{lvl}"]
+        ok = ~na[px]
+        assert np.quantile(np.abs(va.reshape(3, -1)[:, px[ok]] - g[f"map_v_{lvl}"][:, ok]).max(0), 0.999) < 1e-3
+    mine.close()
 
 
 @pytest.mark.parametrize("odometry", [0, 2])
 def test_degenerate_frames_vs_reference_cuda_live(built, frames, odometry):
     """Edge cases the domain has, frame by frame against the reference's CUDA path: depth with holes and sensor noise, a completely
     empty depth frame (no ICP inliers: the 6x6 system is all zeros and the solve must return a zero increment like Eigen's LDLT),
-    a half-empty frame, and a repeated frame (zero motion)."""
+    a half-empty frame, and a repeated frame (zero motion).  The reference's run: tests/golden/ref_degenerate_256.npz (its poses and,
+    ICP-only, a seeded sample of 100 000 of its touched voxels)."""
     import kintinuous_b200 as kb
-    from oracle import refbind
-    if not refbind.RefCuda.available(256):
-        pytest.skip("oracle/_ref not present")
     from kintinuous_b200 import synth
+    g = np.load(os.path.join(GOLDEN, "ref_degenerate_256.npz"))
     rng = np.random.default_rng(11)
     seq = []
     for k in range(8):
@@ -117,20 +116,19 @@ def test_degenerate_frames_vs_reference_cuda_live(built, frames, odometry):
         seq.append((d, c))
     cfg = kb.Config.default(vol=256, odometry=odometry)
     mine = kb.Tracker(cfg)
-    rt = refbind.RefCuda(256).tracker(refbind.TrackerConfig.from_kt(cfg))
     for k, (d, c) in enumerate(seq):
-        p = mine.process_frame(d, c, k); rt.process(d, c, k)
-        Ra, ta, ga, wa = p.as_tuple(); Rb, tb, gb, wb = rt.pose()
+        p = mine.process_frame(d, c, k)
+        Ra, ta, ga, wa = p.as_tuple()
+        gp = g[f"poses_{odometry}"][k]; Rb, tb, wb = gp[:9].reshape(3, 3), gp[9:12], g[f"wraps_{odometry}"][k]
         assert np.isfinite(ta).all() and np.isfinite(Ra).all(), k
         tol = 1e-4 if (odometry == 0 or k < 3) else 2e-3          # photometric odometry is chaotic after a few frames (DESIGN.md section 5)
         assert np.abs(ta - tb).max() <= tol and rot_angle(Ra, Rb) <= tol and (wa == wb).all(), (k, np.abs(ta - tb).max())
-    ta, ca = mine.export_volume(); tb, cb = rt.export_volume()
-    touched = cb[..., 3] != 0
+    ta, ca = mine.export_volume()
     if odometry == 0:
-        d = np.abs(ta.astype(np.int32) - tb.astype(np.int32))[touched]
+        d = np.abs(ta.reshape(-1)[g["vol_idx"]].astype(np.int32) - g["vol_tsdf"].astype(np.int32))
         assert (d <= 1).mean() >= 0.99, float((d <= 1).mean())
-        assert abs(int((ca[..., 3] != 0).sum()) - int(touched.sum())) <= 2e-3 * touched.sum()
-    mine.close(); rt.close()
+        assert abs(int((ca[..., 3] != 0).sum()) - int(g["touched"])) <= 2e-3 * int(g["touched"])
+    mine.close()
 
 
 def test_run_to_run_determinism(built, frames):
@@ -271,13 +269,15 @@ def test_kernel_variants_are_bit_identical(built):
       the reference) versus the default, which prepares the per-pixel colour weight and float RGB once per frame;
     * KT_INT_ZU=1: one voxel per step at 6 CTAs/SM (the default for volumes >= 1024^3);
     * KT_INT_NOBOX=1: integrate launched over the whole volume instead of the frustum's box of storage tiles (kt_frustum.hpp);
+    * KT_ICP_STAGE_PASSES=2: a two-pass shared-memory stage, so that ICP level 0 streams its remaining passes from global memory as
+      1280x960 does on one H100 (kt_icp.cu), versus the full stage;
     * KT_INT_SEQ_REPLAY=1: the running sums of a column replayed one float addition at a time up to its first voxel, as the reference
       does, versus the default exact fast-forward (kt_replay.cuh, replay_add)."""
     import subprocess
     import sys
     from conftest import ROOT
     out = {}
-    for tag, extra in (("default", {}), ("idx64", {"KT_FORCE_IDX64": "1"}), ("noprep", {"KT_INT_PREP": "0"}), ("zu1", {"KT_INT_ZU": "1"}), ("seqreplay", {"KT_INT_SEQ_REPLAY": "1"}), ("nobox", {"KT_INT_NOBOX": "1"}),
+    for tag, extra in (("default", {}), ("idx64", {"KT_FORCE_IDX64": "1"}), ("noprep", {"KT_INT_PREP": "0"}), ("zu1", {"KT_INT_ZU": "1"}), ("seqreplay", {"KT_INT_SEQ_REPLAY": "1"}), ("nobox", {"KT_INT_NOBOX": "1"}), ("stage2", {"KT_ICP_STAGE_PASSES": "2"}),
                        ("idx64_noprep", {"KT_FORCE_IDX64": "1", "KT_INT_PREP": "0"})):
         env = dict(os.environ, PYTHONPATH=ROOT, **extra)
         r = subprocess.run([sys.executable, "-c", _IDX64_SCRIPT], env=env, capture_output=True, text=True, timeout=600, cwd=ROOT)

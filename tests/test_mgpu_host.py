@@ -67,14 +67,16 @@ def test_control_plane_world2_gloo(tmp_path):
 
 
 def test_split_icp_pixel_partition_covers_every_pixel_once():
-    """KT_MG_SPLIT_ICP: world * 148 CTAs split the pixels of every pyramid level; the ranges must tile [0, N) exactly, be 4-pixel aligned (the
-    TMA bulk copies need 16-byte granules) and fit the shared-memory stage the host sizes for them."""
+    """KT_MG_SPLIT_ICP: world * 132 CTAs (one per H100 SM) split the pixels of every pyramid level; the ranges must tile [0, N) exactly and
+    be 4-pixel aligned (the TMA bulk copies need 16-byte granules).  The host stages min(passes, STAGE_MAX_K = 18) passes of a range
+    (kt_icp.cu): 18 passes must fit an H100 block's 227 KB beside the kernel's static shared memory, and only level 0 of 1280x960 on one
+    GPU (19 passes) streams a remainder from global memory."""
     from kintinuous_b200 import mgpu
     for rows, cols in ((480, 640), (960, 1280)):
         for level in range(3):
             n = (rows >> level) * (cols >> level)
             for world in (1, 2, 4, 8):
-                ctas = 148
+                ctas = 132
                 seen = 0
                 worst = 0
                 for rank in range(world):
@@ -84,5 +86,7 @@ def test_split_icp_pixel_partition_covers_every_pixel_once():
                         seen += c
                         worst = max(worst, c)
                 assert seen == n
-                # the stage holds ceil(q / 512) passes of 512 pixels x 6 planes x 4 bytes (kt_icp.cu, STAGE_MAX_K = 17)
-                assert -(-worst // 512) <= 17
+                # the stage holds min(ceil(q / 512), 18) passes of 512 pixels x 6 planes x 4 bytes
+                passes = -(-worst // 512)
+                assert min(passes, 18) * 512 * 6 * 4 <= 227 * 1024 - 4096
+                assert (passes > 18) == ((rows, cols, level, world) == (960, 1280, 0, 1)), (rows, level, world, passes)

@@ -1,5 +1,5 @@
 """Pin the CPU oracle (oracle/kt_oracle_cpu.cpp) against golden vectors produced by the REFERENCE's own CUDA operators
-on a B200 (tools/make_golden.py -> tests/golden/*.npz).  The reference ships no fixtures of its own (SURVEY.md section 4).
+on an H100 (tools/make_golden.py -> tests/golden/*.npz).  The reference ships no fixtures of its own (SURVEY.md section 4).
 
 Tolerances (stated per test): the oracle uses IEEE division / sqrt / expf where the reference's build uses the approximate
 instructions (--prec-div=false --prec-sqrt=false, __expf, rsqrtf), so floating-point maps agree to a few ulp, integer images
@@ -130,15 +130,16 @@ def test_integrate_raycast_extract(cpu_oracle, G, scene):
     tsdf, color, ds0, wrap, vs = _integrate_twice(lib, scene, G, V, trunc)
     assert np.allclose(ds0, G["depth_scaled"], rtol=3e-7, atol=0)          # scaleDepth: sqrt.approx / div.approx vs IEEE
     touched = np.flatnonzero(color.reshape(-1, 4)[:, 3])
-    assert abs(len(touched) - int(G["vol_touched"])) <= 2e-4 * int(G["vol_touched"])
-    idx = G["vol_idx"]
-    dt = np.abs(tsdf[idx].astype(np.int32) - G["vol_tsdf"].astype(np.int32))
+    Gv = np.load(os.path.join(GOLDEN, "ops_160x120_volume.npz"))          # every 4th voxel the reference touched
+    assert abs(len(touched) - int(Gv["vol_touched"])) <= 2e-4 * int(Gv["vol_touched"])
+    idx = Gv["vol_idx"]
+    dt = np.abs(tsdf[idx].astype(np.int32) - Gv["vol_tsdf"].astype(np.int32))
     # TSDF: <= 1 LSB on >= 99.9 % of the reference's touched voxels (a voxel whose projection lands on a pixel boundary may read
     # the neighbouring depth pixel under IEEE vs approximate arithmetic)
     assert (dt <= 1).mean() >= 0.999, float((dt <= 1).mean())
-    dw = color.reshape(-1, 4)[idx, 3].astype(int) - G["vol_color"][:, 3].astype(int)
+    dw = color.reshape(-1, 4)[idx, 3].astype(int) - Gv["vol_color"][:, 3].astype(int)
     assert (dw == 0).mean() >= 0.9995
-    drgb = np.abs(color.reshape(-1, 4)[idx, :3].astype(int) - G["vol_color"][:, :3].astype(int)).max(1)
+    drgb = np.abs(color.reshape(-1, 4)[idx, :3].astype(int) - Gv["vol_color"][:, :3].astype(int)).max(1)
     assert (drgb <= 1).mean() >= 0.995
 
     # raycast the ORACLE volume and compare with the reference's raycast of the REFERENCE volume

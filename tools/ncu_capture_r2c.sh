@@ -3,11 +3,11 @@
 # and the per-iteration odometry kernels of the operator API / large-image fallback (KT_FORCE_PER_ITERATION).   tools/ncu_capture_r2c.sh <tag>
 set -u
 TAG=${1:-r2v3}
-mkdir -p gpurun_out
+mkdir -p prof_out
 cap() {  # name, kernel regex, skip, command...
   local name=$1 k=$2 skip=$3; shift 3
-  timeout 600 ncu --set full --clock-control none --import-source on -k regex:$k -s $skip -c 1 -f -o gpurun_out/prof_${TAG}_$name "$@" > gpurun_out/ncu_${TAG}_$name.log 2>&1
-  tail -1 gpurun_out/ncu_${TAG}_$name.log | cut -c1-160
+  timeout 600 ncu --set full --clock-control none --import-source on -k regex:$k -s $skip -c 1 -f -o prof_out/prof_${TAG}_$name "$@" > prof_out/ncu_${TAG}_$name.log 2>&1
+  tail -1 prof_out/ncu_${TAG}_$name.log | cut -c1-160
 }
 cap slice_bounds_kernel slice_bounds_kernel 0 python tools/prof_shift.py
 cap slice_mark_kernel slice_mark_kernel 0 python tools/prof_shift.py

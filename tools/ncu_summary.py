@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Build the per-kernel table of profiles/r1_ncu_summary.md from the raw ncu exports (profiles/<prefix>_<kernel>.csv).
+"""Print the per-kernel table of the raw ncu exports (prof_out/<prefix>_<kernel>.csv, written by tools/ncu_export.sh).
 usage: ncu_summary.py <prefix>     e.g. r1_ncu_full_v10"""
 import csv, glob, os, sys
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -11,7 +11,7 @@ cols = [("grid x block", None), ("regs", "launch__registers_per_thread"), ("time
         ("top stall (warps per issue)", None)]
 print("| kernel | " + " | ".join(c[0] for c in cols) + " |")
 print("|---|" + "---|" * len(cols))
-for f in sorted(glob.glob(os.path.join(ROOT, "profiles", prefix + "_*.csv"))):
+for f in sorted(glob.glob(os.path.join(ROOT, "prof_out", prefix + "_*.csv"))):
     rows = list(csv.reader(open(f)))
     H, U, V = rows[0], rows[1], rows[2]
     def g(n, unit=True):

@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Per-kernel fingerprint of the DEVICE code of the product library: md5 of each kernel's SASS instruction stream with addresses,
-encodings and the path-dependent anonymous-namespace hash stripped.  profiles/r1_sass_fingerprint.txt holds the fingerprints of the build
-that last passed `pytest -m gpu` on a B200; host-only edits, comment edits and explicit re-statements of what the compiler already
+encodings and the path-dependent anonymous-namespace hash stripped.  Compared with the fingerprints of a build that passed
+`pytest -m gpu`, host-only edits, comment edits and explicit re-statements of what the compiler already
 generated must leave a kernel's line unchanged (tools/sass_diff.py shows what changed inside a kernel).
 usage: sass_fingerprint.py [build-dir]   (default kintinuous_b200/csrc/build)"""
 import glob, hashlib, os, re, subprocess, sys

@@ -1,7 +1,7 @@
 // Micro-benchmark (development tool, not product): the per-iteration TAIL of the whole-frame odometry kernels in isolation --
 // "every CTA contributes 29 floats, every CTA ends up with the 29 grid totals and the solved pose" -- in several designs, timed in SM
 // cycles per iteration from CTA 0 over many iterations, one CTA of 512 threads per SM like icp_frame_kernel.
-//   nvcc -O3 -std=c++17 -gencode arch=compute_100a,code=sm_100a -I kintinuous_b200/csrc tools/tail_bench.cu -o gpurun_out/tail_bench
+//   nvcc -O3 -std=c++17 -gencode arch=compute_90a,code=sm_90a -I kintinuous_b200/csrc tools/tail_bench.cu -o tools/bin/tail_bench   (tools/bin/ is git-ignored)
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
