@@ -88,6 +88,14 @@ typedef struct kt_point_xyzrgbnormal {
     float pad[2];
 } kt_point_xyzrgbnormal;
 
+/* 32-byte mesh vertex (kt_op_mesh_volume, kt_get_slice_mesh): position in the slice frame (metres, as kt_point_xyzrgb), unit normal
+ * towards increasing TSDF (free space; (0,0,0) when degenerate), colour and alpha = weight of the voxel nearer the surface. */
+typedef struct kt_mesh_vertex {
+    float x, y, z, nx, ny, nz;
+    uint8_t r, g, b, a;
+    uint32_t _pad;
+} kt_mesh_vertex;
+
 typedef struct kt_ctx kt_ctx;
 
 KT_API const char* kt_last_error(void);
@@ -130,6 +138,24 @@ KT_API int kt_get_processed_slice(kt_ctx* ctx, int idx, kt_point_xyzrgbnormal* p
 /* The rest of the CloudSlice record (CloudSlice.h:47-60): which odometry produced the pose (CloudSlice::Odometry: 0 ICP, 2 RGBD --
  * KintinuousTracker.cpp:137-176,565: the kind of the active OdometryProvider), the camera pose at hand-over (volume-global
  * translation, row-major rotation) and the frame's timestamp. */
+/* Meshing on the device, standing in for MeshGenerator (backend/MeshGenerator.cpp:37-191 the meshing thread, :193-227 calculateMesh,
+ * :229-280 save).  The reference triangulates every slice's processed cloud with PCL's greedy projection on the CPU; here each slice is
+ * meshed by marching cubes over the TSDF box it was extracted from, before that box is cleared (kt_op_mesh_volume below: no parity with
+ * PCL).  When enabled, every slice recorded from now on carries a mesh (weight_cull: corners need alpha >= weight_cull, -cw, default
+ * 8); the FINAL slice of kt_finalise meshes the whole volume.  Neighbouring slices overlap by the overlap planes, so their meshes
+ * repeat the triangles there (as the reference's merged export with default flags keeps its overlap).  kt_get_slice_mesh copies up to
+ * max_verts / max_tris and returns both counts; it waits for that slice's download only, and returns KT_ERR_STATE for a slice recorded
+ * with meshing off.  A volume shared by several GPUs (world > 1) cannot be meshed: KT_ERR_INVALID. */
+KT_API int kt_set_slice_meshing(kt_ctx* ctx, int enabled, int weight_cull);
+KT_API int kt_get_slice_mesh(kt_ctx* ctx, int idx, kt_mesh_vertex* verts, size_t max_verts, uint32_t* tris, size_t max_tris,
+                             size_t* n_verts, size_t* n_tris);
+/* The whole volume's mesh at this moment, synchronous, without recording a slice (the live mesh of PangoVis.cpp:395), with the weight
+ * cull of kt_set_slice_meshing (8 until it is called); copies up to the capacities, returns both counts.  world > 1: KT_ERR_INVALID. */
+KT_API int kt_get_live_mesh(kt_ctx* ctx, kt_mesh_vertex* verts, size_t max_verts, uint32_t* tris, size_t max_tris, size_t* n_verts, size_t* n_tris);
+/* MeshGenerator::save's "merging for export" branch (:229-280): every recorded slice mesh in order, indices offset, as one binary
+ * little-endian PLY (vertex: float x y z nx ny nz, uchar red green blue; face: list uchar int vertex_indices).  KT_ERR_STATE when no
+ * recorded slice has a mesh. */
+KT_API int kt_save_mesh_ply(kt_ctx* ctx, const char* path);
 typedef struct kt_slice_info { int dimension; int odometry; float camera_t[3]; float camera_R[9]; uint64_t utime; size_t count; } kt_slice_info;
 KT_API int kt_get_slice_info(kt_ctx* ctx, int idx, kt_slice_info* info);
 /* Dense pose graph (KintinuousTracker::DensePose / densePoseGraph / latestDensePoseId, KintinuousTracker.h:151-172): one record per
@@ -249,6 +275,19 @@ KT_API int kt_op_extract_slice(const int16_t* tsdf_dev, const float* volume_size
  * filter in that case). */
 KT_API int kt_op_process_slice(const kt_point_xyzrgb* points_dev, size_t n, int weight_cull, float leaf, int k_search,
                                kt_point_xyzrgbnormal* out_dev, size_t capacity, size_t* count, void* stream);
+/* Marching cubes over the cells of the logical box [minX,maxX) x [minY,maxY) x [minZ,maxZ) of the cyclic volume, with extractCloudSlice's
+ * addressing (voxel_wrap3: storage offset, any value, reduced mod vol; real_voxel_wrap3: global offset of the positions).  Stands in
+ * for calculateMesh (backend/MeshGenerator.cpp:193-227; a different algorithm, no parity with PCL's greedy projection).  A corner is
+ * valid when extractCloudSlice would use it (W != 0, F != 1) and W >= weight_cull; inside when its raw TSDF is < 0.  A cell (lower corner
+ * in the box, upper corner < vol on every axis, no cyclic wrap) is meshed when its 8 corners are valid and not all on one side.  Output
+ * (device): one vertex per crossing edge of a meshed cell, at exactly the point extractCloudSlice emits for that edge, ordered by the
+ * edge's lower voxel (x fastest) then axis; triangles as uint32 triples, ordered by cell then case-table order, (v1-v0)x(v2-v0) pointing
+ * to free space.  Deterministic, independent of the launch and of voxel_wrap3.  The counts are always returned; if either output is
+ * too small the call returns KT_ERR_CAPACITY and writes neither. */
+KT_API int kt_op_mesh_volume(const int16_t* tsdf_dev, const uint8_t* color_dev, int vol, const float* volume_size3,
+                             const int* voxel_wrap3, const int* real_voxel_wrap3, int minX, int maxX, int minY, int maxY, int minZ, int maxZ,
+                             int weight_cull, kt_mesh_vertex* verts_dev, size_t max_verts, uint32_t* tris_dev, size_t max_tris,
+                             size_t* n_verts, size_t* n_tris, void* stream);
 /* clearVolume{X,Y,Z}[Back] + ...c on both volumes (tsdf_volume.cu:117-448). axis 0..2, back 0/1. */
 KT_API int kt_op_clear_volume(int axis, int back, int16_t* tsdf_dev, uint8_t* color_dev, int vol, int current_wrap, int delta_wrap, void* stream);
 /* initVolume + initColorVolume (tsdf_volume.cu:469, :77) */

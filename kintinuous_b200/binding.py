@@ -91,6 +91,11 @@ assert POINT_DTYPE.itemsize == 32
 POINT_NORMAL_DTYPE = np.dtype([("x", "<f4"), ("y", "<f4"), ("z", "<f4"), ("_p0", "<f4"), ("nx", "<f4"), ("ny", "<f4"), ("nz", "<f4"), ("_p1", "<f4"),
                                ("b", "u1"), ("g", "u1"), ("r", "u1"), ("a", "u1"), ("curvature", "<f4"), ("_p2", "<f4", (2,))])
 assert POINT_NORMAL_DTYPE.itemsize == 48
+# kt_mesh_vertex (32 bytes): position, unit normal, colour, alpha = weight
+MESH_VERTEX_DTYPE = np.dtype([("x", "<f4"), ("y", "<f4"), ("z", "<f4"), ("nx", "<f4"), ("ny", "<f4"), ("nz", "<f4"),
+                              ("r", "u1"), ("g", "u1"), ("b", "u1"), ("a", "u1"), ("_pad", "<u4")])
+assert MESH_VERTEX_DTYPE.itemsize == 32
+KT_ERR_CAPACITY = -4
 
 
 def _ptr(a):
@@ -196,6 +201,31 @@ class Tracker:
         if n.value:
             _check(self.lib.kt_get_processed_slice(self.h, idx, _ptr(pts), C.c_size_t(n.value), C.byref(n)))
         return pts
+
+    def set_slice_meshing(self, enabled=True, weight_cull=8):
+        """Marching-cubes mesh of every slice recorded from now on (kt_set_slice_meshing)."""
+        _check(self.lib.kt_set_slice_meshing(self.h, int(enabled), int(weight_cull)))
+
+    def get_slice_mesh(self, idx):
+        """(vertices MESH_VERTEX_DTYPE [n], triangles uint32 [m, 3]) of slice idx."""
+        nv = C.c_size_t(0); nt = C.c_size_t(0)
+        _check(self.lib.kt_get_slice_mesh(self.h, idx, None, C.c_size_t(0), None, C.c_size_t(0), C.byref(nv), C.byref(nt)))
+        v = np.zeros(nv.value, MESH_VERTEX_DTYPE); t = np.zeros((nt.value, 3), np.uint32)
+        _check(self.lib.kt_get_slice_mesh(self.h, idx, _ptr(v), C.c_size_t(len(v)), _ptr(t), C.c_size_t(len(t)), C.byref(nv), C.byref(nt)))
+        return v, t
+
+    def live_mesh(self):
+        """Mesh of the whole volume now (kt_get_live_mesh): (vertices, triangles)."""
+        nv = C.c_size_t(0); nt = C.c_size_t(0)
+        _check(self.lib.kt_get_live_mesh(self.h, None, C.c_size_t(0), None, C.c_size_t(0), C.byref(nv), C.byref(nt)))
+        v = np.zeros(nv.value, MESH_VERTEX_DTYPE); t = np.zeros((nt.value, 3), np.uint32)
+        _check(self.lib.kt_get_live_mesh(self.h, _ptr(v), C.c_size_t(len(v)), _ptr(t), C.c_size_t(len(t)), C.byref(nv), C.byref(nt)))
+        assert (nv.value, nt.value) == (len(v), len(t))
+        return v, t
+
+    def save_mesh_ply(self, path):
+        """Every recorded slice mesh, concatenated, as a binary PLY (kt_save_mesh_ply)."""
+        _check(self.lib.kt_save_mesh_ply(self.h, os.fsencode(path)))
 
     def slice_info(self, idx):
         """The rest of the CloudSlice record: dimension, odometry kind, camera pose at hand-over, timestamp, point count."""
@@ -387,6 +417,32 @@ class _Ops:
         _check(self._l().kt_op_process_slice(_ptr(points_dev), C.c_size_t(n), int(weight_cull), C.c_float(leaf), int(k_search), _ptr(out_dev), C.c_size_t(capacity),
                                              C.byref(cnt), None))
         return cnt.value
+
+    def mesh_volume_into(self, tsdf, color, vol, volume_size, wrap, real_wrap, box, weight_cull, verts_dev, max_verts, tris_dev, max_tris):
+        """kt_op_mesh_volume into caller buffers: (status, n_verts, n_tris); status is 0 or KT_ERR_CAPACITY (nothing written)."""
+        vs = _f(volume_size)
+        w = np.ascontiguousarray(np.asarray(wrap, dtype=np.int32)); rw = np.ascontiguousarray(np.asarray(real_wrap, dtype=np.int32))
+        nv = C.c_size_t(0); nt = C.c_size_t(0)
+        st = self._l().kt_op_mesh_volume(_ptr(tsdf), _ptr(color), vol, _ptr(vs), _ptr(w), _ptr(rw), box[0], box[1], box[2], box[3], box[4], box[5],
+                                         int(weight_cull), _ptr(verts_dev), C.c_size_t(max_verts), _ptr(tris_dev), C.c_size_t(max_tris),
+                                         C.byref(nv), C.byref(nt), None)
+        if st not in (0, KT_ERR_CAPACITY):
+            _check(st)
+        return st, nv.value, nt.value
+
+    def mesh_volume(self, tsdf, color, vol, volume_size, wrap, real_wrap, box, weight_cull=8):
+        """Marching cubes over box (minX, maxX, minY, maxY, minZ, maxZ) of a device volume: counts first, then output buffers of
+        exactly that size.  Returns host arrays (vertices MESH_VERTEX_DTYPE [n], triangles uint32 [m, 3])."""
+        import torch
+        st, nv, nt = self.mesh_volume_into(tsdf, color, vol, volume_size, wrap, real_wrap, box, weight_cull, None, 0, None, 0)
+        if st == 0:
+            return np.zeros(0, MESH_VERTEX_DTYPE), np.zeros((0, 3), np.uint32)
+        v = torch.empty(nv * 32, dtype=torch.uint8, device="cuda")
+        t = torch.empty(max(nt, 1) * 3, dtype=torch.int32, device="cuda")
+        st, nv2, nt2 = self.mesh_volume_into(tsdf, color, vol, volume_size, wrap, real_wrap, box, weight_cull, v, nv, t, nt)
+        _check(st)
+        assert (nv2, nt2) == (nv, nt)
+        return v.cpu().numpy().view(MESH_VERTEX_DTYPE).copy(), t[:3 * nt].cpu().numpy().view(np.uint32).reshape(nt, 3).copy()
 
     def clear_volume(self, axis, back, tsdf, color, vol, current, delta):
         _check(self._l().kt_op_clear_volume(axis, back, _ptr(tsdf), _ptr(color), vol, current, delta, None))

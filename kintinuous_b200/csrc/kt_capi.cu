@@ -19,7 +19,8 @@ cudaStream_t st(void* s) { return (cudaStream_t)s; }
 // either: internal.h:299-536 has static state in computeDerivativeImages and __device__ globals in extract.cu).  One set PER DEVICE
 // (the device current at the call), and the calls that use it are serialised by a process-wide mutex, so operator calls from several
 // host threads / on several devices are safe, just not concurrent.
-struct OpScratch { OdomState* state; float* partials; int* ipartials; float* ztable; int ztable_n; unsigned int* counter; OdomState* host_state; SliceWorkspace slice_ws; };
+struct OpScratch { OdomState* state; float* partials; int* ipartials; float* ztable; int ztable_n; unsigned int* counter; OdomState* host_state; SliceWorkspace slice_ws;
+                   MeshWorkspace mesh_ws; };
 enum { KT_MAX_DEVICES = 64 };
 OpScratch g_ops_dev[KT_MAX_DEVICES];
 std::mutex g_ops_mu;
@@ -184,6 +185,26 @@ int kt_op_process_slice(const kt_point_xyzrgb* points_dev, size_t n, int weight_
 {
     KT_OPS_LOCK();
     return process_slice(points_dev, n, weight_cull, leaf, k_search, out_dev, capacity, count, &g_ops.slice_ws, st(s));
+}
+
+int kt_op_mesh_volume(const int16_t* tsdf, const uint8_t* color, int vol, const float* vs, const int* wrap, const int* real_wrap,
+                      int minX, int maxX, int minY, int maxY, int minZ, int maxZ, int weight_cull, kt_mesh_vertex* verts, size_t max_verts,
+                      uint32_t* tris, size_t max_tris, size_t* n_verts, size_t* n_tris, void* s)
+{
+    if (!tsdf || !color || !vs || !wrap || !real_wrap || !n_verts || !n_tris || vol <= 0) { set_error("kt_op_mesh_volume: bad argument"); return KT_ERR_INVALID; }
+    if (minX < 0 || minY < 0 || minZ < 0 || maxX > vol || maxY > vol || maxZ > vol) { set_error("kt_op_mesh_volume: box outside [0, vol]"); return KT_ERR_INVALID; }
+    KT_OPS_LOCK();
+    MeshArgs a;
+    a.tsdf = tsdf; a.color = color; a.vol = vol; a.volume_size = make_float3(vs[0], vs[1], vs[2]);
+    a.wrap = make_int3(wrap[0], wrap[1], wrap[2]); a.real_wrap = make_int3(real_wrap[0], real_wrap[1], real_wrap[2]);
+    a.minX = minX; a.maxX = maxX; a.minY = minY; a.maxY = maxY; a.minZ = minZ; a.maxZ = maxZ; a.weight_cull = weight_cull;
+    size_t nv = 0, nt = 0;
+    int r = mesh_count(a, &g_ops.mesh_ws, &nv, &nt, st(s)); if (r) return r;
+    *n_verts = nv; *n_tris = nt;
+    if (nv > max_verts || nt > max_tris) { set_error("kt_op_mesh_volume: %zu vertices / %zu triangles exceed the capacities", nv, nt); return KT_ERR_CAPACITY; }
+    r = mesh_emit(a, &g_ops.mesh_ws, nv, verts, tris, st(s)); if (r) return r;
+    KT_CUDA(cudaStreamSynchronize(st(s)));
+    return KT_OK;
 }
 
 int kt_op_clear_volume(int axis, int back, int16_t* tsdf, uint8_t* color, int vol, int current, int delta, void* s)

@@ -167,6 +167,23 @@ struct SliceWorkspace { unsigned int* mask; unsigned int* word_off; unsigned int
 int process_slice(const void* points_dev /* kt_point_xyzrgb */, size_t n, int weight_cull, float leaf, int k_search, void* out_dev /* kt_point_xyzrgbnormal */,
                   size_t capacity, size_t* count, SliceWorkspace* ws, cudaStream_t s);
 void slice_ws_free(SliceWorkspace* ws);
+// ---- marching cubes over a box of the cyclic volume (kt_mesh.cu): an indexed mesh in a fixed order, see the file header ----
+struct MeshArgs {
+    const int16_t* tsdf; const uint8_t* color; int vol; float3 volume_size; int3 wrap; int3 real_wrap;   // wrap / real_wrap: as extract_slice
+    int minX, maxX, minY, maxY, minZ, maxZ; int weight_cull;
+};
+struct MeshWorkspace {
+    unsigned long long* counts; size_t counts_cap;    // per-tile vertex / triangle totals and their exclusive scans
+    void* tmp; size_t tmp_cap;                        // CUB scan storage
+    unsigned long long* keys; size_t keys_cap;        // 3 * owner + axis of every vertex, ascending
+    unsigned long long* totals_host;                  // pinned: vertex and triangle counts
+    MeshWorkspace() : counts(0), counts_cap(0), tmp(0), tmp_cap(0), keys(0), keys_cap(0), totals_host(0) {}
+};
+// count + scan, then one read-back (synchronises s): the mesh's vertex and triangle counts
+int mesh_count(const MeshArgs& a, MeshWorkspace* ws, size_t* n_verts, size_t* n_tris, cudaStream_t s);
+// after mesh_count with the same arguments: writes n_verts 32-byte kt_mesh_vertex records and the triangles (3 x uint32 each); asynchronous
+int mesh_emit(const MeshArgs& a, MeshWorkspace* ws, size_t n_verts, void* verts, uint32_t* tris, cudaStream_t s);
+void mesh_ws_free(MeshWorkspace* ws);
 // cross-GPU barrier: every rank writes `epoch` into slot [rank] of every peer's flag array, then waits until all slots of its own
 // array reach `epoch` (bounded spin: returns through *error_dev != 0 instead of hanging the GPU if a peer never arrives)
 int xgpu_barrier(unsigned int* const* peer_flags_dev /* [world] device array of pointers */, unsigned int* my_flags, int rank, int world,

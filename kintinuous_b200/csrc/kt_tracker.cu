@@ -84,6 +84,7 @@ static Mat33 to_mat33(const float* m) { Mat33 r; r.r0 = make_float3(m[0], m[1], 
 // `ready` fires when the bytes have landed.  The reference downloads into a pageable std::vector with a blocking cudaMemcpy inside
 // processFrame (KintinuousTracker.cpp:1166, containers/device_memory.cpp:146-157).
 struct SliceRec { int dimension; kt_point_xyzrgb* points; size_t count; kt_point_xyzrgbnormal* processed; size_t processed_count; bool has_processed;
+                  kt_mesh_vertex* mesh_verts; uint32_t* mesh_tris; size_t mesh_nv, mesh_nt; bool has_mesh;
                   cudaEvent_t ready; float camera_t[3]; float camera_R[9]; uint64_t utime; };
 
 // Pinned host memory handed out in slabs (one cudaHostAlloc per 64 MB, not per slice); everything is released together by kt_reset.
@@ -152,6 +153,9 @@ struct kt_ctx {
     PinnedArena* slice_arena; cudaStream_t stream_slices; cudaEvent_t ev_cloud_ready, ev_cloud_free; bool cloud_busy;
     // CloudSliceProcessor on the device (kt_slice.cu): weight cull + voxel grid + normals of every slice before it leaves the GPU
     int slice_processing, slice_weight_cull; SliceWorkspace slice_ws; kt_point_xyzrgbnormal* proc_dev; size_t proc_count;
+    // marching cubes of every slice's box before it is cleared (kt_mesh.cu); buffers grow at a shift, downloaded with the slice
+    int slice_meshing, mesh_weight_cull; MeshWorkspace mesh_ws; kt_mesh_vertex* mesh_verts_dev; uint32_t* mesh_tris_dev;
+    size_t mesh_verts_cap, mesh_tris_cap, mesh_nv, mesh_nt;
     // RGB-D
     float* lastDepth[LEVELS]; float* nextDepth[LEVELS]; uint8_t* lastImage[LEVELS]; uint8_t* nextImage[LEVELS];
     int16_t* nextdIdx[LEVELS]; int16_t* nextdIdy[LEVELS]; float* pointClouds[LEVELS]; void* corresImg[LEVELS];
@@ -212,6 +216,41 @@ int fetch_cloud(kt_ctx* c, const int* vWrapCopy, const int* lo, const int* hi)  
     return 0;
 }
 
+// Marching cubes over the box [lo, hi) that fetch_cloud has just extracted, on the tracker stream and before the box is cleared, into
+// the context's mesh buffers (grown here: the count is read back first, once).  MeshGenerator::calculateMesh (MeshGenerator.cpp:193-227)
+// on the device, by a different algorithm (kt_mesh.cu).
+int mesh_box(kt_ctx* c, const int* vWrapCopy, const int* lo, const int* hi)
+{
+    // the previous slice's asynchronous download may still be reading the mesh buffers
+    if (c->cloud_busy) { KT_CUDA(cudaStreamWaitEvent(c->stream, c->ev_cloud_free, 0)); c->cloud_busy = false; }
+    MeshArgs a;
+    a.tsdf = c->tsdf; a.color = c->color; a.vol = c->cfg.vol; a.volume_size = make_float3(c->size, c->size, c->size);
+    a.wrap = make_int3(vWrapCopy[0], vWrapCopy[1], vWrapCopy[2]); a.real_wrap = make_int3(c->voxelWrap[0], c->voxelWrap[1], c->voxelWrap[2]);
+    a.minX = lo[0]; a.maxX = hi[0]; a.minY = lo[1]; a.maxY = hi[1]; a.minZ = lo[2]; a.maxZ = hi[2]; a.weight_cull = c->mesh_weight_cull;
+    size_t nv = 0, nt = 0;
+    int r = mesh_count(a, &c->mesh_ws, &nv, &nt, c->stream); if (r) return r;
+    if (nv > c->mesh_verts_cap || nt > c->mesh_tris_cap) {
+        KT_CUDA(cudaStreamSynchronize(c->stream_slices));
+        if (nv > c->mesh_verts_cap) {
+            if (c->mesh_verts_dev) cudaFree(c->mesh_verts_dev);
+            c->mesh_verts_dev = 0; c->mesh_verts_cap = 0;
+            const size_t want = nv + nv / 4 + 1024;
+            KT_CUDA(cudaMalloc((void**)&c->mesh_verts_dev, want * sizeof(kt_mesh_vertex)));
+            c->mesh_verts_cap = want;
+        }
+        if (nt > c->mesh_tris_cap) {
+            if (c->mesh_tris_dev) cudaFree(c->mesh_tris_dev);
+            c->mesh_tris_dev = 0; c->mesh_tris_cap = 0;
+            const size_t want = nt + nt / 4 + 1024;
+            KT_CUDA(cudaMalloc((void**)&c->mesh_tris_dev, want * 3 * sizeof(uint32_t)));
+            c->mesh_tris_cap = want;
+        }
+    }
+    r = mesh_emit(a, &c->mesh_ws, nv, c->mesh_verts_dev, c->mesh_tris_dev, c->stream); if (r) return r;
+    c->mesh_nv = nv; c->mesh_nt = nt;
+    return 0;
+}
+
 // mutexOutCloudBuffer (KintinuousTracker.cpp:1156-1208): record the extracted cloud as a CloudSlice.  The points go to pinned host
 // memory with an ASYNCHRONOUS copy on a side stream -- the frame's clear / integrate / ray cast do not wait for it; readers of the slice
 // do (kt_get_slice waits on the slice's event).  With slice processing on, the slice is culled, voxel-gridded and given normals on the
@@ -219,6 +258,8 @@ int fetch_cloud(kt_ctx* c, const int* vWrapCopy, const int* lo, const int* hi)  
 int push_slice(kt_ctx* c, int dimension)
 {
     SliceRec s; s.dimension = dimension; s.points = 0; s.count = c->cloud_count; s.processed = 0; s.processed_count = 0; s.has_processed = false; s.ready = 0;
+    s.has_mesh = c->slice_meshing != 0; s.mesh_verts = 0; s.mesh_tris = 0;
+    s.mesh_nv = s.has_mesh ? c->mesh_nv : 0; s.mesh_nt = s.has_mesh ? c->mesh_nt : 0;
     c->proc_count = 0;
     if (c->slice_processing && c->cloud_count) {
         if (!c->proc_dev) { void* q = 0; KT_CUDA(cudaMalloc(&q, c->cloud_capacity * sizeof(kt_point_xyzrgbnormal))); c->allocs.push_back(q); c->proc_dev = (kt_point_xyzrgbnormal*)q; }
@@ -227,15 +268,21 @@ int push_slice(kt_ctx* c, int dimension)
     }
     s.has_processed = c->slice_processing != 0;
     s.processed_count = c->proc_count;
-    if (c->cloud_count) {
-        s.points = (kt_point_xyzrgb*)c->slice_arena->alloc(c->cloud_count * sizeof(kt_point_xyzrgb));
+    if (c->cloud_count || s.mesh_nv) {
+        if (c->cloud_count) s.points = (kt_point_xyzrgb*)c->slice_arena->alloc(c->cloud_count * sizeof(kt_point_xyzrgb));
         if (c->proc_count) s.processed = (kt_point_xyzrgbnormal*)c->slice_arena->alloc(c->proc_count * sizeof(kt_point_xyzrgbnormal));
-        if (!s.points || (c->proc_count && !s.processed)) { set_error("pinned host memory for a slice of %zu points", c->cloud_count); return KT_ERR_CUDA; }
+        if (s.mesh_nv) s.mesh_verts = (kt_mesh_vertex*)c->slice_arena->alloc(s.mesh_nv * sizeof(kt_mesh_vertex));
+        if (s.mesh_nt) s.mesh_tris = (uint32_t*)c->slice_arena->alloc(s.mesh_nt * 3 * sizeof(uint32_t));
+        if ((c->cloud_count && !s.points) || (c->proc_count && !s.processed) || (s.mesh_nv && !s.mesh_verts) || (s.mesh_nt && !s.mesh_tris)) {
+            set_error("pinned host memory for a slice of %zu points", c->cloud_count); return KT_ERR_CUDA;
+        }
         KT_CUDA(cudaEventCreateWithFlags(&s.ready, cudaEventDisableTiming));
         KT_CUDA(cudaEventRecord(c->ev_cloud_ready, c->stream));
         KT_CUDA(cudaStreamWaitEvent(c->stream_slices, c->ev_cloud_ready, 0));
-        KT_CUDA(cudaMemcpyAsync(s.points, c->cloud_dev, c->cloud_count * sizeof(kt_point_xyzrgb), cudaMemcpyDeviceToHost, c->stream_slices));
+        if (c->cloud_count) KT_CUDA(cudaMemcpyAsync(s.points, c->cloud_dev, c->cloud_count * sizeof(kt_point_xyzrgb), cudaMemcpyDeviceToHost, c->stream_slices));
         if (c->proc_count) KT_CUDA(cudaMemcpyAsync(s.processed, c->proc_dev, c->proc_count * sizeof(kt_point_xyzrgbnormal), cudaMemcpyDeviceToHost, c->stream_slices));
+        if (s.mesh_nv) KT_CUDA(cudaMemcpyAsync(s.mesh_verts, c->mesh_verts_dev, s.mesh_nv * sizeof(kt_mesh_vertex), cudaMemcpyDeviceToHost, c->stream_slices));
+        if (s.mesh_nt) KT_CUDA(cudaMemcpyAsync(s.mesh_tris, c->mesh_tris_dev, s.mesh_nt * 3 * sizeof(uint32_t), cudaMemcpyDeviceToHost, c->stream_slices));
         KT_CUDA(cudaEventRecord(s.ready, c->stream_slices));
         KT_CUDA(cudaEventRecord(c->ev_cloud_free, c->stream_slices));
         c->cloud_busy = true;
@@ -510,6 +557,7 @@ int process_frame_device(kt_ctx* c, uint64_t utime, kt_pose* out)
         const bool cycled = dir != 0;
         if (cycled) {
             if ((r = fetch_cloud(c, vWrapCopy, lo, hi))) return r;
+            if (c->slice_meshing && (r = mesh_box(c, vWrapCopy, lo, hi))) return r;
             if ((r = mg_barrier(c))) return r;                          // peers may still read my boundary plane for their extraction
             if ((r = clear_volume_shared(axis, dir < 0 ? 1 : 0, c->vv, V, c->voxelWrap[axis], c->voxelWrap[axis] + n, c->stream))) return r;
         }
@@ -724,6 +772,7 @@ int kt_create(const kt_config* cfg, kt_ctx** out)
     c->cloud_capacity = (size_t)c->cfg.cloud_capacity;
     KT_TRY(dev_alloc(c, &c->cloud_dev, c->cloud_capacity)); KT_TRY(dev_alloc(c, &c->counter_dev, 1));
     c->slice_arena = new PinnedArena();
+    c->mesh_weight_cull = 8;                                   // -cw default, also the live mesh's until kt_set_slice_meshing
     if (!c->slice_arena->alloc(256)) { set_error("kt_create: pinned slice arena"); kt_destroy(c); return KT_ERR_CUDA; }      // the first 64 MB slab now, not inside the first shift frame
     c->slice_arena->rewind();
     KT_TRY(kt::cuda_check(cudaStreamCreateWithFlags(&c->stream_slices, cudaStreamNonBlocking), "stream_slices", __FILE__, __LINE__));
@@ -758,6 +807,9 @@ int kt_destroy(kt_ctx* c)
     if (c->pose_log) fclose(c->pose_log);
     if (c->slice_arena) { c->slice_arena->release(); delete c->slice_arena; }
     slice_ws_free(&c->slice_ws);
+    mesh_ws_free(&c->mesh_ws);
+    if (c->mesh_verts_dev) cudaFree(c->mesh_verts_dev);
+    if (c->mesh_tris_dev) cudaFree(c->mesh_tris_dev);
     if (c->stream_slices) cudaStreamDestroy(c->stream_slices);
     if (c->ev_cloud_ready) cudaEventDestroy(c->ev_cloud_ready);
     if (c->ev_cloud_free) cudaEventDestroy(c->ev_cloud_free);
@@ -872,6 +924,7 @@ int kt_finalise(kt_ctx* c)                                                      
     int lo[3] = {0, 0, 0}, hi[3] = {V, V, V};
     int r = fetch_cloud(c, vWrapCopy, lo, hi);
     if (r) return r;
+    if (c->slice_meshing && (r = mesh_box(c, vWrapCopy, lo, hi))) return r;
     return push_slice(c, 7);     // CloudSlice::FINAL
 }
 
@@ -947,6 +1000,88 @@ int kt_get_processed_slice(kt_ctx* c, int idx, kt_point_xyzrgbnormal* points, si
         KT_CUDA(cudaEventSynchronize(s.ready));
         std::memcpy(points, s.processed, n * sizeof(kt_point_xyzrgbnormal));
     }
+    return KT_OK;
+}
+
+int kt_set_slice_meshing(kt_ctx* c, int enabled, int weight_cull)
+{
+    if (!c) return KT_ERR_INVALID;
+    if (c->world > 1 && enabled) { set_error("kt_set_slice_meshing: a volume shared by %d GPUs cannot be meshed", c->world); return KT_ERR_INVALID; }
+    c->slice_meshing = enabled != 0; c->mesh_weight_cull = weight_cull;
+    return KT_OK;
+}
+
+int kt_get_slice_mesh(kt_ctx* c, int idx, kt_mesh_vertex* verts, size_t max_verts, uint32_t* tris, size_t max_tris, size_t* n_verts, size_t* n_tris)
+{
+    if (!c || idx < 0 || idx >= (int)c->slices.size()) { set_error("kt_get_slice_mesh: bad index"); return KT_ERR_INVALID; }
+    const SliceRec& s = c->slices[idx];
+    if (!s.has_mesh) { set_error("kt_get_slice_mesh: slice %d was recorded with meshing off (kt_set_slice_meshing)", idx); return KT_ERR_STATE; }
+    if (n_verts) *n_verts = s.mesh_nv;
+    if (n_tris) *n_tris = s.mesh_nt;
+    const size_t nv = verts ? std::min(max_verts, s.mesh_nv) : 0, nt = tris ? std::min(max_tris, s.mesh_nt) : 0;
+    if (nv || nt) KT_CUDA(cudaEventSynchronize(s.ready));
+    if (nv) std::memcpy(verts, s.mesh_verts, nv * sizeof(kt_mesh_vertex));
+    if (nt) std::memcpy(tris, s.mesh_tris, nt * 3 * sizeof(uint32_t));
+    return KT_OK;
+}
+
+int kt_get_live_mesh(kt_ctx* c, kt_mesh_vertex* verts, size_t max_verts, uint32_t* tris, size_t max_tris, size_t* n_verts, size_t* n_tris)
+{
+    if (!c) return KT_ERR_INVALID;
+    if (c->world > 1) { set_error("kt_get_live_mesh: a volume shared by %d GPUs cannot be meshed", c->world); return KT_ERR_INVALID; }
+    KT_CUDA(cudaSetDevice(c->cfg.device));
+    int vWrapCopy[3]; vwrap_copy(c, vWrapCopy);
+    const int V = c->cfg.vol;
+    int lo[3] = {0, 0, 0}, hi[3] = {V, V, V};
+    int r = mesh_box(c, vWrapCopy, lo, hi);
+    if (r) return r;
+    if (n_verts) *n_verts = c->mesh_nv;
+    if (n_tris) *n_tris = c->mesh_nt;
+    const size_t nv = verts ? std::min(max_verts, c->mesh_nv) : 0, nt = tris ? std::min(max_tris, c->mesh_nt) : 0;
+    if (nv) KT_CUDA(cudaMemcpyAsync(verts, c->mesh_verts_dev, nv * sizeof(kt_mesh_vertex), cudaMemcpyDeviceToHost, c->stream));
+    if (nt) KT_CUDA(cudaMemcpyAsync(tris, c->mesh_tris_dev, nt * 3 * sizeof(uint32_t), cudaMemcpyDeviceToHost, c->stream));
+    KT_CUDA(cudaStreamSynchronize(c->stream));
+    return KT_OK;
+}
+
+int kt_save_mesh_ply(kt_ctx* c, const char* path)
+{
+    if (!c || !path) return KT_ERR_INVALID;
+    size_t nv = 0, nt = 0; bool any = false;
+    for (const auto& s : c->slices) if (s.has_mesh) { any = true; nv += s.mesh_nv; nt += s.mesh_nt; }
+    if (!any) { set_error("kt_save_mesh_ply: no slice was recorded with meshing on (kt_set_slice_meshing)"); return KT_ERR_STATE; }
+    if (nv > 0x7fffffffu) { set_error("kt_save_mesh_ply: %zu vertices do not fit the PLY's int indices", nv); return KT_ERR_CAPACITY; }
+    FILE* f = fopen(path, "wb");
+    if (!f) { set_error("kt_save_mesh_ply: cannot open %s", path); return KT_ERR_INVALID; }
+    fprintf(f, "ply\nformat binary_little_endian 1.0\nelement vertex %zu\nproperty float x\nproperty float y\nproperty float z\n"
+               "property float nx\nproperty float ny\nproperty float nz\nproperty uchar red\nproperty uchar green\nproperty uchar blue\n"
+               "element face %zu\nproperty list uchar int vertex_indices\nend_header\n", nv, nt);
+    std::vector<unsigned char> buf;
+    bool ok = true;
+    for (const auto& s : c->slices) {                              // x86 / aarch64 hosts are little-endian: records are the raw bytes
+        if (!s.has_mesh || !s.mesh_nv) continue;
+        if (cudaEventSynchronize(s.ready) != cudaSuccess) { ok = false; break; }
+        buf.resize(s.mesh_nv * 27);
+        for (size_t i = 0; i < s.mesh_nv; ++i) {
+            std::memcpy(&buf[i * 27], &s.mesh_verts[i].x, 24);
+            buf[i * 27 + 24] = s.mesh_verts[i].r; buf[i * 27 + 25] = s.mesh_verts[i].g; buf[i * 27 + 26] = s.mesh_verts[i].b;
+        }
+        ok = ok && fwrite(buf.data(), 1, buf.size(), f) == buf.size();
+    }
+    uint32_t base = 0;
+    for (const auto& s : c->slices) {
+        if (!ok) break;
+        if (!s.has_mesh) continue;
+        buf.resize(s.mesh_nt * 13);
+        for (size_t t = 0; t < s.mesh_nt; ++t) {
+            buf[t * 13] = 3;
+            for (int k = 0; k < 3; ++k) { const int32_t v = (int32_t)(s.mesh_tris[3 * t + k] + base); std::memcpy(&buf[t * 13 + 1 + 4 * k], &v, 4); }
+        }
+        ok = ok && fwrite(buf.data(), 1, buf.size(), f) == buf.size();
+        base += (uint32_t)s.mesh_nv;
+    }
+    if (fclose(f) != 0) ok = false;
+    if (!ok) { set_error("kt_save_mesh_ply: writing %s failed", path); return KT_ERR_CUDA; }
     return KT_OK;
 }
 
