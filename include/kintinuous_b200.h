@@ -164,6 +164,42 @@ KT_API int kt_get_slice_info(kt_ctx* ctx, int idx, kt_slice_info* info);
 typedef struct kt_dense_pose { uint64_t timestamp; float pose[16]; int is_loop_pose; } kt_dense_pose;
 KT_API int kt_num_dense_poses(kt_ctx* ctx);                                /* latestDensePoseId */
 KT_API int kt_get_dense_pose(kt_ctx* ctx, int idx, kt_dense_pose* out);    /* densePoseGraph.at(idx) */
+/* Map deformation to a corrected trajectory: the embedded deformation graph of the reference's backend (backend/Deformation.cpp:173-346
+ * addCameraLoop, backend/DeformationGraph.cpp) on the GPU.  Loop detection and the pose-graph solve (iSAM) stay with the caller: it passes
+ * the corrected camera poses, each with a timestamp that is in the dense pose graph (else KT_ERR_INVALID), and optional point constraints
+ * (its loop-closure inliers: time, position in the map as tracked, where it belongs).
+ *   - Nodes: the dense pose graph's camera positions, the first and then every one more than node_spacing from the last taken
+ *     (initialiseGraphPoses, DeformationGraph.cpp:51-86; the reference's -dg, default 0.8 m), joined sequentially (connectGraphSeq).
+ *     Fewer than 5 nodes: KT_ERR_STATE.
+ *   - Constraints: each corrected pose pulls the tracked camera position at its time to the corrected one (positions only, as the
+ *     reference); each point constraint pulls its source to its target.
+ *   - Gauss-Newton (optimiseGraphSparse, :714-774): at most 10 steps; no step at all when |r_con| / constraints < 0.1.
+ *   - The map is every processed slice (kt_set_slice_processing) and every slice mesh (kt_set_slice_meshing) recorded so far; a vertex's
+ *     time is its slice's.  The deformed copies are kept in new pinned memory (kt_get_deformed_slice / _mesh); the recorded slices are not
+ *     modified.  Every call deforms the original map from scratch with the constraints it is given -- the reference deforms its map in
+ *     place, loop closure after loop closure.
+ * KT_ERR_STATE with neither processed slices nor meshes; KT_ERR_INVALID for a volume shared by several GPUs (world > 1) and for a
+ * corrected translation, point source or point target that is not finite. */
+typedef struct kt_deform_constraint { uint64_t time; float source[3]; float target[3]; } kt_deform_constraint;
+typedef struct kt_deform_report {
+    int nodes, constraints;
+    int band;                   /* widest node-id span of a term, in 12 x 12 blocks of J^T J (at most 19) */
+    int iterations;             /* Gauss-Newton steps taken */
+    double initial_error;       /* |r|^2 before the first step */
+    double final_error;         /* |r|^2 after the last one */
+    double constraint_error;    /* |r_con| / constraints before the first step (the early-out test: < 0.1) */
+    int deformed;               /* 0: the map is returned unchanged (early-out or failed factorisation) */
+    int solver_failed;          /* 1: a pivot of the Cholesky factorisation was not positive */
+} kt_deform_report;
+KT_API int kt_deform_map(kt_ctx* ctx, const kt_dense_pose* corrected, size_t n, const kt_deform_constraint* points, size_t n_points,
+                         float node_spacing, kt_deform_report* report);
+/* The deformed processed cloud / mesh vertices of slice idx as of the last kt_deform_map (the triangles are kt_get_slice_mesh's).  Copy
+ * up to the capacity, return the count.  KT_ERR_STATE for a slice recorded after that call or without a processed cloud / mesh. */
+KT_API int kt_get_deformed_slice(kt_ctx* ctx, int idx, kt_point_xyzrgbnormal* points, size_t max_points, size_t* count);
+KT_API int kt_get_deformed_slice_mesh(kt_ctx* ctx, int idx, kt_mesh_vertex* verts, size_t max_verts, size_t* n_verts);
+/* The "_opt" mesh of Deformation::saveMesh (Deformation.cpp:85-100): kt_save_mesh_ply's layout over the deformed vertices of the slices
+ * covered by the last kt_deform_map.  KT_ERR_STATE before any kt_deform_map or when none of those slices has a mesh. */
+KT_API int kt_save_deformed_mesh_ply(kt_ctx* ctx, const char* path);
 /* KintinuousTracker::outputPose (.cpp:199-218, :911-914): append one line per tracked frame to `path` ("<saveFile>.poses" in the
  * reference: "utime/1e6 gx gy gz qx qy qz qw").  NULL closes the log.  kt_format_pose_line formats one such line into buf. */
 KT_API int kt_set_pose_log(kt_ctx* ctx, const char* path);
@@ -288,6 +324,27 @@ KT_API int kt_op_mesh_volume(const int16_t* tsdf_dev, const uint8_t* color_dev, 
                              const int* voxel_wrap3, const int* real_voxel_wrap3, int minX, int maxX, int minY, int maxY, int minZ, int maxZ,
                              int weight_cull, kt_mesh_vertex* verts_dev, size_t max_verts, uint32_t* tris_dev, size_t max_tris,
                              size_t* n_verts, size_t* n_tris, void* stream);
+/* Deformation graph operators (kt_deform_map runs the three in turn).  Nodes: n_nodes float xyz positions and their uint64 times,
+ * ascending (device).  kind: 0 = kt_point_xyzrgbnormal, 1 = kt_mesh_vertex, 2 = packed float xyz (weights only).
+ * kt_op_deform_weights -- weightVerticesSeq (DeformationGraph.cpp:441-556): per point, the node nearest its time by binary search (a time
+ * outside the node times clamps to the first / last node; the reference reads past both ends there), the 20 consecutive candidates from
+ * it (back, topped up forward), the k+1 = 5 nearest (float distances, ties by id), weights (1 - |v - g_j| / dMax)^2 in FP64 for the 4
+ * nearest, normalised; out: 4 int32 node ids ascending and their 4 FP64 weights per point.  Fewer than 5 nodes: KT_ERR_STATE. */
+KT_API int kt_op_deform_weights(const float* node_pos_dev, const uint64_t* node_times_dev, int n_nodes, const void* points_dev, int kind,
+                                const uint64_t* times_dev, size_t n, int32_t* ids_dev, double* weights_dev, void* stream);
+/* optimiseGraphSparse (DeformationGraph.cpp:714-774) over the sequentially connected nodes (connectGraphSeq :217-271, k = 4) with one
+ * position constraint per row of con_src (float xyz, device) -> con_dst (double xyz, device), weighted by kt_op_deform_weights' output
+ * for the sources.  Out: 12 doubles per node (rotation column-major, then translation; the identity when report->deformed is 0) and the
+ * report.  The normal equations are solved on the device by a block-banded Cholesky; a term spanning more than 19 node blocks returns
+ * KT_ERR_INVALID. */
+KT_API int kt_op_deform_optimise(const float* node_pos_dev, int n_nodes, const float* con_src_dev, const double* con_dst_dev,
+                                 const int32_t* con_ids_dev, const double* con_weights_dev, size_t n_con, double* params_dev,
+                                 kt_deform_report* report, void* stream);
+/* applyGraphToVertices / computeVertexPosition (DeformationGraph.cpp:644-677, :1028-1054): kind 0 or 1 records from in_dev to out_dev,
+ * position sum_j w_j (R_j (v - g_j) + g_j + t_j), normal sum_j w_j R_j^-T n normalised (zero stays zero), FP64 written as float, every
+ * other byte copied. */
+KT_API int kt_op_deform_apply(const float* node_pos_dev, const double* params_dev, int n_nodes, const int32_t* ids_dev,
+                              const double* weights_dev, const void* in_dev, void* out_dev, int kind, size_t n, void* stream);
 /* clearVolume{X,Y,Z}[Back] + ...c on both volumes (tsdf_volume.cu:117-448). axis 0..2, back 0/1. */
 KT_API int kt_op_clear_volume(int axis, int back, int16_t* tsdf_dev, uint8_t* color_dev, int vol, int current_wrap, int delta_wrap, void* stream);
 /* initVolume + initColorVolume (tsdf_volume.cu:469, :77) */

@@ -70,6 +70,21 @@ class DensePose(C.Structure):
     _fields_ = [("timestamp", C.c_uint64), ("pose", C.c_float * 16), ("is_loop_pose", C.c_int)]
 
 
+class DeformConstraint(C.Structure):
+    """kt_deform_constraint: a point that belongs elsewhere (time, position in the map as tracked, target)."""
+    _fields_ = [("time", C.c_uint64), ("source", C.c_float * 3), ("target", C.c_float * 3)]
+
+
+class DeformReport(C.Structure):
+    """kt_deform_report of kt_deform_map / kt_op_deform_optimise."""
+    _fields_ = [("nodes", C.c_int), ("constraints", C.c_int), ("band", C.c_int), ("iterations", C.c_int),
+                ("initial_error", C.c_double), ("final_error", C.c_double), ("constraint_error", C.c_double),
+                ("deformed", C.c_int), ("solver_failed", C.c_int)]
+
+    def as_dict(self):
+        return {k: getattr(self, k) for k, _ in self._fields_}
+
+
 class SliceInfo(C.Structure):
     _fields_ = [("dimension", C.c_int), ("odometry", C.c_int), ("camera_t", C.c_float * 3), ("camera_R", C.c_float * 9),
                 ("utime", C.c_uint64), ("count", C.c_size_t)]
@@ -226,6 +241,43 @@ class Tracker:
     def save_mesh_ply(self, path):
         """Every recorded slice mesh, concatenated, as a binary PLY (kt_save_mesh_ply)."""
         _check(self.lib.kt_save_mesh_ply(self.h, os.fsencode(path)))
+
+    def deform_map(self, corrected, points=(), node_spacing=0.8):
+        """Deform every processed slice and slice mesh recorded so far to a corrected trajectory (kt_deform_map).  corrected: iterable
+        of (timestamp, 4x4 pose) with timestamps from the dense pose graph; points: iterable of (time, source xyz, target xyz).
+        Returns the DeformReport."""
+        corrected = list(corrected); points = list(points)
+        cp = (DensePose * max(len(corrected), 1))()
+        for i, (ts, pose) in enumerate(corrected):
+            cp[i].timestamp = int(ts); cp[i].pose[:] = [float(v) for v in np.asarray(pose, np.float32).reshape(16)]
+        pp = (DeformConstraint * max(len(points), 1))()
+        for i, (ts, src, dst) in enumerate(points):
+            pp[i].time = int(ts); pp[i].source[:] = [float(v) for v in src]; pp[i].target[:] = [float(v) for v in dst]
+        rep = DeformReport()
+        _check(self.lib.kt_deform_map(self.h, cp, C.c_size_t(len(corrected)), pp, C.c_size_t(len(points)), C.c_float(node_spacing), C.byref(rep)))
+        return rep
+
+    def get_deformed_slice(self, idx):
+        """Processed cloud of slice idx as deformed by the last deform_map (POINT_NORMAL_DTYPE)."""
+        n = C.c_size_t(0)
+        _check(self.lib.kt_get_deformed_slice(self.h, idx, None, C.c_size_t(0), C.byref(n)))
+        pts = np.zeros(n.value, dtype=POINT_NORMAL_DTYPE)
+        if n.value:
+            _check(self.lib.kt_get_deformed_slice(self.h, idx, _ptr(pts), C.c_size_t(n.value), C.byref(n)))
+        return pts
+
+    def get_deformed_slice_mesh(self, idx):
+        """Mesh vertices of slice idx as deformed by the last deform_map (MESH_VERTEX_DTYPE); the triangles are get_slice_mesh's."""
+        n = C.c_size_t(0)
+        _check(self.lib.kt_get_deformed_slice_mesh(self.h, idx, None, C.c_size_t(0), C.byref(n)))
+        v = np.zeros(n.value, dtype=MESH_VERTEX_DTYPE)
+        if n.value:
+            _check(self.lib.kt_get_deformed_slice_mesh(self.h, idx, _ptr(v), C.c_size_t(n.value), C.byref(n)))
+        return v
+
+    def save_deformed_mesh_ply(self, path):
+        """The deformed slice meshes of the last deform_map as one binary PLY (kt_save_deformed_mesh_ply)."""
+        _check(self.lib.kt_save_deformed_mesh_ply(self.h, os.fsencode(path)))
 
     def slice_info(self, idx):
         """The rest of the CloudSlice record: dimension, odometry kind, camera pose at hand-over, timestamp, point count."""
@@ -443,6 +495,25 @@ class _Ops:
         _check(st)
         assert (nv2, nt2) == (nv, nt)
         return v.cpu().numpy().view(MESH_VERTEX_DTYPE).copy(), t[:3 * nt].cpu().numpy().view(np.uint32).reshape(nt, 3).copy()
+
+    def deform_weights(self, node_pos, node_times, points, kind, times, ids, weights):
+        """kt_op_deform_weights: node_pos float32 [n, 3], node_times uint64 [n] (as int64 tensors), points (kind 0
+        POINT_NORMAL records, 1 MESH_VERTEX records, 2 float32 xyz), times [N]; writes ids int32 [N, 4] and weights float64 [N, 4]."""
+        _check(self._l().kt_op_deform_weights(_ptr(node_pos), _ptr(node_times), int(node_pos.shape[0]), _ptr(points), int(kind), _ptr(times),
+                                              C.c_size_t(int(times.shape[0])), _ptr(ids), _ptr(weights), None))
+
+    def deform_optimise(self, node_pos, con_src, con_dst, con_ids, con_weights, params):
+        """kt_op_deform_optimise: con_src float32 [m, 3], con_dst float64 [m, 3], the sources' ids / weights; writes params float64
+        [n, 12] (rotation column-major, translation).  Returns the DeformReport."""
+        rep = DeformReport()
+        _check(self._l().kt_op_deform_optimise(_ptr(node_pos), int(node_pos.shape[0]), _ptr(con_src), _ptr(con_dst), _ptr(con_ids),
+                                               _ptr(con_weights), C.c_size_t(int(con_src.shape[0])), _ptr(params), C.byref(rep), None))
+        return rep
+
+    def deform_apply(self, node_pos, params, ids, weights, points_in, points_out, kind, n):
+        """kt_op_deform_apply: n records of kind 0 (POINT_NORMAL) / 1 (MESH_VERTEX) from points_in to points_out."""
+        _check(self._l().kt_op_deform_apply(_ptr(node_pos), _ptr(params), int(node_pos.shape[0]), _ptr(ids), _ptr(weights), _ptr(points_in),
+                                            _ptr(points_out), int(kind), C.c_size_t(int(n)), None))
 
     def clear_volume(self, axis, back, tsdf, color, vol, current, delta):
         _check(self._l().kt_op_clear_volume(axis, back, _ptr(tsdf), _ptr(color), vol, current, delta, None))

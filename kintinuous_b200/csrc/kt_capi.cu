@@ -6,6 +6,7 @@
 #include <cstring>
 #include <cstddef>
 #include <mutex>
+#include <vector>
 
 using namespace kt;
 
@@ -203,6 +204,42 @@ int kt_op_mesh_volume(const int16_t* tsdf, const uint8_t* color, int vol, const 
     *n_verts = nv; *n_tris = nt;
     if (nv > max_verts || nt > max_tris) { set_error("kt_op_mesh_volume: %zu vertices / %zu triangles exceed the capacities", nv, nt); return KT_ERR_CAPACITY; }
     r = mesh_emit(a, &g_ops.mesh_ws, nv, verts, tris, st(s)); if (r) return r;
+    KT_CUDA(cudaStreamSynchronize(st(s)));
+    return KT_OK;
+}
+
+int kt_op_deform_weights(const float* node_pos, const uint64_t* node_times, int n_nodes, const void* pts, int kind, const uint64_t* times,
+                         size_t n, int32_t* ids, double* weights, void* s)
+{
+    if (!node_pos || !node_times || (n && (!pts || !times || !ids || !weights))) { set_error("kt_op_deform_weights: bad argument"); return KT_ERR_INVALID; }
+    int r = deform_weights(node_pos, node_times, n_nodes, pts, kind, times, n, ids, weights, st(s)); if (r) return r;
+    KT_CUDA(cudaStreamSynchronize(st(s)));
+    return KT_OK;
+}
+
+int kt_op_deform_optimise(const float* node_pos, int n_nodes, const float* con_src, const double* con_dst, const int32_t* con_ids,
+                          const double* con_w, size_t m, double* params, kt_deform_report* report, void* s)
+{
+    if (!node_pos || !params || !report || n_nodes < 0 || (m && (!con_src || !con_dst || !con_ids || !con_w))) {
+        set_error("kt_op_deform_optimise: bad argument"); return KT_ERR_INVALID;
+    }
+    std::vector<float> pos((size_t)n_nodes * 3), src(m * 3); std::vector<double> dst(m * 3), w(m * 4); std::vector<int32_t> ids(m * 4);
+    KT_CUDA(cudaMemcpyAsync(pos.data(), node_pos, pos.size() * sizeof(float), cudaMemcpyDeviceToHost, st(s)));
+    if (m) {
+        KT_CUDA(cudaMemcpyAsync(src.data(), con_src, src.size() * sizeof(float), cudaMemcpyDeviceToHost, st(s)));
+        KT_CUDA(cudaMemcpyAsync(dst.data(), con_dst, dst.size() * sizeof(double), cudaMemcpyDeviceToHost, st(s)));
+        KT_CUDA(cudaMemcpyAsync(ids.data(), con_ids, ids.size() * sizeof(int32_t), cudaMemcpyDeviceToHost, st(s)));
+        KT_CUDA(cudaMemcpyAsync(w.data(), con_w, w.size() * sizeof(double), cudaMemcpyDeviceToHost, st(s)));
+    }
+    KT_CUDA(cudaStreamSynchronize(st(s)));
+    return deform_optimise(pos.data(), n_nodes, src.data(), dst.data(), ids.data(), w.data(), m, params, report, st(s));
+}
+
+int kt_op_deform_apply(const float* node_pos, const double* params, int n_nodes, const int32_t* ids, const double* weights, const void* in,
+                       void* out, int kind, size_t n, void* s)
+{
+    if (!node_pos || !params || n_nodes <= 0 || (n && (!ids || !weights || !in || !out))) { set_error("kt_op_deform_apply: bad argument"); return KT_ERR_INVALID; }
+    int r = deform_apply(node_pos, params, n_nodes, ids, weights, in, out, kind, n, st(s)); if (r) return r;
     KT_CUDA(cudaStreamSynchronize(st(s)));
     return KT_OK;
 }

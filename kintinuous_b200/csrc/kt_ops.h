@@ -3,6 +3,8 @@
 #pragma once
 #include "kt_common.cuh"
 
+struct kt_deform_report;
+
 namespace kt {
 
 static const int LEVELS = 4;                 // ICPOdometry.h:52 / RGBDOdometry.h:96
@@ -184,6 +186,19 @@ int mesh_count(const MeshArgs& a, MeshWorkspace* ws, size_t* n_verts, size_t* n_
 // after mesh_count with the same arguments: writes n_verts 32-byte kt_mesh_vertex records and the triangles (3 x uint32 each); asynchronous
 int mesh_emit(const MeshArgs& a, MeshWorkspace* ws, size_t n_verts, void* verts, uint32_t* tris, cudaStream_t s);
 void mesh_ws_free(MeshWorkspace* ws);
+// ---- embedded deformation graph (kt_deform.cu, host logic in kt_deform.hpp) ----
+// Node positions: float n x 3 (device), node times ascending.  kind: 0 kt_point_xyzrgbnormal, 1 kt_mesh_vertex, 2 packed float xyz.
+// Writes 4 node ids (int32, ascending) and 4 FP64 weights per point; asynchronous.
+int deform_weights(const float* node_pos, const uint64_t* node_times, int n_nodes, const void* pts, int kind, const uint64_t* times, size_t n,
+                   int32_t* ids, double* weights, cudaStream_t s);
+// Gauss-Newton over the graph (host arrays: node positions, constraint sources / targets and their ids / weights); writes the 12
+// unknowns per node (rotation column-major, translation) to x_dev -- the identity unless rep->deformed -- and every field of the
+// report.  Synchronises s.
+int deform_optimise(const float* node_pos, int n_nodes, const float* src, const double* dst, const int32_t* ids, const double* weights, size_t m,
+                    double* x_dev, kt_deform_report* rep, cudaStream_t s);
+// Deforms n records of kind 0 / 1 from in to out (may not alias) with the nodes' unknowns x; asynchronous.
+int deform_apply(const float* node_pos, const double* x, int n_nodes, const int32_t* ids, const double* weights, const void* in, void* out,
+                 int kind, size_t n, cudaStream_t s);
 // cross-GPU barrier: every rank writes `epoch` into slot [rank] of every peer's flag array, then waits until all slots of its own
 // array reach `epoch` (bounded spin: returns through *error_dev != 0 instead of hanging the GPU if a peer never arrives)
 int xgpu_barrier(unsigned int* const* peer_flags_dev /* [world] device array of pointers */, unsigned int* my_flags, int rank, int world,

@@ -15,6 +15,7 @@
 #include "kt_ops.h"
 #include "kt_shift.hpp"
 #include "kt_posegraph.hpp"
+#include "kt_deform.hpp"
 #include <cstdlib>
 #include "../../include/kintinuous_b200.h"
 #include <vector>
@@ -156,6 +157,10 @@ struct kt_ctx {
     // marching cubes of every slice's box before it is cleared (kt_mesh.cu); buffers grow at a shift, downloaded with the slice
     int slice_meshing, mesh_weight_cull; MeshWorkspace mesh_ws; kt_mesh_vertex* mesh_verts_dev; uint32_t* mesh_tris_dev;
     size_t mesh_verts_cap, mesh_tris_cap, mesh_nv, mesh_nt;
+    // the map as deformed by the last kt_deform_map (kt_deform.cu): one record per slice recorded before that call, in its own pinned
+    // arena, or the slice's own buffers when the call left the map unchanged
+    struct Deformed { kt_point_xyzrgbnormal* processed; kt_mesh_vertex* mesh_verts; };
+    std::vector<Deformed> deformed; PinnedArena* deform_arena;
     // RGB-D
     float* lastDepth[LEVELS]; float* nextDepth[LEVELS]; uint8_t* lastImage[LEVELS]; uint8_t* nextImage[LEVELS];
     int16_t* nextdIdx[LEVELS]; int16_t* nextdIdy[LEVELS]; float* pointClouds[LEVELS]; void* corresImg[LEVELS];
@@ -642,6 +647,8 @@ int kt_reset(kt_ctx* c)
     c->tvecs.push_back(tb);
     for (int i = 0; i < 3; ++i) { c->voxelWrap[i] = 0; c->currentGlobalCamera[i] = c->volumeBasis[i] - c->size * 0.5f; }
     drop_slices(c);
+    c->deformed.clear();
+    if (c->deform_arena) c->deform_arena->rewind();
     c->dense_poses.clear();                      // reset(): densePoseGraph.clear(), latestDensePoseId = 0 (.cpp:300-301)
     c->trace_iters = 0; c->shifted_last = 0; c->cloud_count = 0;
     c->pf_valid = false; c->pf_built = false; c->frontend_ready = false; c->maps_on_stream = false;
@@ -806,6 +813,7 @@ int kt_destroy(kt_ctx* c)
     drop_slices(c);
     if (c->pose_log) fclose(c->pose_log);
     if (c->slice_arena) { c->slice_arena->release(); delete c->slice_arena; }
+    if (c->deform_arena) { c->deform_arena->release(); delete c->deform_arena; }
     slice_ws_free(&c->slice_ws);
     mesh_ws_free(&c->mesh_ws);
     if (c->mesh_verts_dev) cudaFree(c->mesh_verts_dev);
@@ -1044,32 +1052,35 @@ int kt_get_live_mesh(kt_ctx* c, kt_mesh_vertex* verts, size_t max_verts, uint32_
     return KT_OK;
 }
 
-int kt_save_mesh_ply(kt_ctx* c, const char* path)
+// The meshes of the first n_slices slices as one binary PLY; with `deformed`, the vertices of the last kt_deform_map
+static int save_mesh_ply(kt_ctx* c, const char* path, size_t n_slices, bool deformed, const char* who)
 {
-    if (!c || !path) return KT_ERR_INVALID;
     size_t nv = 0, nt = 0; bool any = false;
-    for (const auto& s : c->slices) if (s.has_mesh) { any = true; nv += s.mesh_nv; nt += s.mesh_nt; }
-    if (!any) { set_error("kt_save_mesh_ply: no slice was recorded with meshing on (kt_set_slice_meshing)"); return KT_ERR_STATE; }
-    if (nv > 0x7fffffffu) { set_error("kt_save_mesh_ply: %zu vertices do not fit the PLY's int indices", nv); return KT_ERR_CAPACITY; }
+    for (size_t i = 0; i < n_slices; ++i) { const auto& s = c->slices[i]; if (s.has_mesh) { any = true; nv += s.mesh_nv; nt += s.mesh_nt; } }
+    if (!any) { set_error("%s: no slice was recorded with meshing on (kt_set_slice_meshing)", who); return KT_ERR_STATE; }
+    if (nv > 0x7fffffffu) { set_error("%s: %zu vertices do not fit the PLY's int indices", who, nv); return KT_ERR_CAPACITY; }
     FILE* f = fopen(path, "wb");
-    if (!f) { set_error("kt_save_mesh_ply: cannot open %s", path); return KT_ERR_INVALID; }
+    if (!f) { set_error("%s: cannot open %s", who, path); return KT_ERR_INVALID; }
     fprintf(f, "ply\nformat binary_little_endian 1.0\nelement vertex %zu\nproperty float x\nproperty float y\nproperty float z\n"
                "property float nx\nproperty float ny\nproperty float nz\nproperty uchar red\nproperty uchar green\nproperty uchar blue\n"
                "element face %zu\nproperty list uchar int vertex_indices\nend_header\n", nv, nt);
     std::vector<unsigned char> buf;
     bool ok = true;
-    for (const auto& s : c->slices) {                              // x86 / aarch64 hosts are little-endian: records are the raw bytes
+    for (size_t k = 0; k < n_slices; ++k) {                        // x86 / aarch64 hosts are little-endian: records are the raw bytes
+        const auto& s = c->slices[k];
         if (!s.has_mesh || !s.mesh_nv) continue;
         if (cudaEventSynchronize(s.ready) != cudaSuccess) { ok = false; break; }
+        const kt_mesh_vertex* mv = deformed ? c->deformed[k].mesh_verts : s.mesh_verts;
         buf.resize(s.mesh_nv * 27);
         for (size_t i = 0; i < s.mesh_nv; ++i) {
-            std::memcpy(&buf[i * 27], &s.mesh_verts[i].x, 24);
-            buf[i * 27 + 24] = s.mesh_verts[i].r; buf[i * 27 + 25] = s.mesh_verts[i].g; buf[i * 27 + 26] = s.mesh_verts[i].b;
+            std::memcpy(&buf[i * 27], &mv[i].x, 24);
+            buf[i * 27 + 24] = mv[i].r; buf[i * 27 + 25] = mv[i].g; buf[i * 27 + 26] = mv[i].b;
         }
         ok = ok && fwrite(buf.data(), 1, buf.size(), f) == buf.size();
     }
     uint32_t base = 0;
-    for (const auto& s : c->slices) {
+    for (size_t k = 0; k < n_slices; ++k) {
+        const auto& s = c->slices[k];
         if (!ok) break;
         if (!s.has_mesh) continue;
         buf.resize(s.mesh_nt * 13);
@@ -1081,8 +1092,167 @@ int kt_save_mesh_ply(kt_ctx* c, const char* path)
         base += (uint32_t)s.mesh_nv;
     }
     if (fclose(f) != 0) ok = false;
-    if (!ok) { set_error("kt_save_mesh_ply: writing %s failed", path); return KT_ERR_CUDA; }
+    if (!ok) { set_error("%s: writing %s failed", who, path); return KT_ERR_CUDA; }
     return KT_OK;
+}
+
+int kt_save_mesh_ply(kt_ctx* c, const char* path)
+{
+    if (!c || !path) return KT_ERR_INVALID;
+    return save_mesh_ply(c, path, c->slices.size(), false, "kt_save_mesh_ply");
+}
+
+// Deformation::addCameraLoop's graph work (Deformation.cpp:264-318: appendVertices, the camera-pose constraints, optimiseGraphSparse,
+// applyGraphToVertices) over the map recorded so far, on the tracker's stream.  Nothing the tracker reads is written.
+int kt_deform_map(kt_ctx* c, const kt_dense_pose* corrected, size_t n, const kt_deform_constraint* points, size_t n_points, float node_spacing,
+                  kt_deform_report* report)
+{
+    if (!c || !report || (n && !corrected) || (n_points && !points) || !(node_spacing >= 0.f)) { set_error("kt_deform_map: bad argument"); return KT_ERR_INVALID; }
+    std::memset(report, 0, sizeof(*report));
+    if (c->world > 1) { set_error("kt_deform_map: a volume shared by %d GPUs cannot be deformed", c->world); return KT_ERR_INVALID; }
+    size_t np = 0, nm = 0; bool any = false;
+    for (const auto& s : c->slices) {
+        if (s.has_processed) { any = true; np += s.processed_count; }
+        if (s.has_mesh) { any = true; nm += s.mesh_nv; }
+    }
+    if (!any) { set_error("kt_deform_map: no processed slice and no slice mesh recorded (kt_set_slice_processing / kt_set_slice_meshing)"); return KT_ERR_STATE; }
+    // nodes: the dense pose graph's positions (initialiseGraphPoses)
+    const size_t nd = c->dense_poses.size();
+    std::vector<float> gpos(nd * 3); std::vector<uint64_t> gtime(nd);
+    for (size_t i = 0; i < nd; ++i) {
+        gtime[i] = c->dense_poses[i].timestamp;
+        for (int e = 0; e < 3; ++e) gpos[3 * i + e] = c->dense_poses[i].pose[4 * e + 3];
+    }
+    const std::vector<int> take = deform_sample_nodes(gpos.data(), nd, node_spacing);
+    const int nn = (int)take.size();
+    if (nn < DEFORM_K + 1) {
+        set_error("kt_deform_map: node_spacing %g m leaves %d graph nodes on the trajectory; at least %d are needed", (double)node_spacing, nn, DEFORM_K + 1);
+        return KT_ERR_STATE;
+    }
+    std::vector<float> npos(3 * (size_t)nn); std::vector<uint64_t> ntime(nn);
+    for (int j = 0; j < nn; ++j) { ntime[j] = gtime[take[j]]; for (int e = 0; e < 3; ++e) npos[3 * j + e] = gpos[3 * take[j] + e]; }
+    for (int j = 1; j < nn; ++j)
+        if (ntime[j] < ntime[j - 1]) { set_error("kt_deform_map: the dense pose graph's timestamps are not ascending"); return KT_ERR_STATE; }
+    // constraints: corrected camera positions, then the caller's points
+    std::vector<uint64_t> ctime(n); std::vector<double> cpos(3 * n);
+    for (size_t i = 0; i < n; ++i) { ctime[i] = corrected[i].timestamp; for (int e = 0; e < 3; ++e) cpos[3 * i + e] = corrected[i].pose[4 * e + 3]; }
+    std::vector<DeformConstraint> cons;
+    const long miss = deform_pose_constraints(gtime.data(), gpos.data(), nd, ctime.data(), cpos.data(), n, cons);
+    if (miss >= 0) { set_error("kt_deform_map: corrected pose %ld has timestamp %llu, which is not in the dense pose graph", miss, (unsigned long long)ctime[miss]); return KT_ERR_INVALID; }
+    for (size_t i = 0; i < n_points; ++i) {
+        DeformConstraint q; q.time = points[i].time;
+        for (int e = 0; e < 3; ++e) { q.src[e] = points[i].source[e]; q.dst[e] = points[i].target[e]; }
+        cons.push_back(q);
+    }
+    const size_t m = cons.size();
+    if (!m) { set_error("kt_deform_map: no constraints"); return KT_ERR_INVALID; }
+    for (size_t l = 0; l < m; ++l)
+        if (deform_first_non_finite(cons[l].src, 3) >= 0 || deform_first_non_finite(cons[l].dst, 3) >= 0) {
+            if (l < n) set_error("kt_deform_map: corrected pose %zu has a translation that is not finite", l);
+            else set_error("kt_deform_map: point constraint %zu has a source or target that is not finite", l - n);
+            return KT_ERR_INVALID;
+        }
+    std::vector<float> csrc(3 * m); std::vector<double> cdst(3 * m); std::vector<uint64_t> ct(m);
+    for (size_t l = 0; l < m; ++l) { ct[l] = cons[l].time; for (int e = 0; e < 3; ++e) { csrc[3 * l + e] = cons[l].src[e]; cdst[3 * l + e] = cons[l].dst[e]; } }
+
+    KT_CUDA(cudaSetDevice(c->cfg.device));
+    if (c->stream_slices) KT_CUDA(cudaStreamSynchronize(c->stream_slices));           // every slice has landed in its pinned buffers
+    const size_t nmax = std::max(std::max(np, nm), m);
+    float* d_npos = 0; uint64_t* d_ntime = 0; double* d_x = 0; uint64_t* d_t = 0; int32_t* d_ids = 0; double* d_w = 0; void* d_in = 0; void* d_out = 0;
+    auto cleanup = [&]() { cudaFree(d_npos); cudaFree(d_ntime); cudaFree(d_x); cudaFree(d_t); cudaFree(d_ids); cudaFree(d_w); cudaFree(d_in); cudaFree(d_out); };
+    auto run = [&]() -> int {
+        cudaStream_t s = c->stream;
+        KT_CUDA(cudaMalloc((void**)&d_npos, npos.size() * sizeof(float)));
+        KT_CUDA(cudaMalloc((void**)&d_ntime, ntime.size() * sizeof(uint64_t)));
+        KT_CUDA(cudaMalloc((void**)&d_x, (size_t)nn * 12 * sizeof(double)));
+        KT_CUDA(cudaMalloc((void**)&d_t, nmax * sizeof(uint64_t)));
+        KT_CUDA(cudaMalloc((void**)&d_ids, nmax * 4 * sizeof(int32_t)));
+        KT_CUDA(cudaMalloc((void**)&d_w, nmax * 4 * sizeof(double)));
+        KT_CUDA(cudaMalloc(&d_in, nmax * sizeof(kt_point_xyzrgbnormal)));
+        KT_CUDA(cudaMemcpyAsync(d_npos, npos.data(), npos.size() * sizeof(float), cudaMemcpyHostToDevice, s));
+        KT_CUDA(cudaMemcpyAsync(d_ntime, ntime.data(), ntime.size() * sizeof(uint64_t), cudaMemcpyHostToDevice, s));
+        // constraint weights (their sources are vertices of the graph too: appendVertices) -> optimiseGraphSparse
+        KT_CUDA(cudaMemcpyAsync(d_in, csrc.data(), csrc.size() * sizeof(float), cudaMemcpyHostToDevice, s));
+        KT_CUDA(cudaMemcpyAsync(d_t, ct.data(), m * sizeof(uint64_t), cudaMemcpyHostToDevice, s));
+        int r = deform_weights(d_npos, d_ntime, nn, d_in, 2, d_t, m, d_ids, d_w, s); if (r) return r;
+        std::vector<int32_t> cids(4 * m); std::vector<double> cw(4 * m);
+        KT_CUDA(cudaMemcpyAsync(cids.data(), d_ids, cids.size() * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
+        KT_CUDA(cudaMemcpyAsync(cw.data(), d_w, cw.size() * sizeof(double), cudaMemcpyDeviceToHost, s));
+        KT_CUDA(cudaStreamSynchronize(s));
+        r = deform_optimise(npos.data(), nn, csrc.data(), cdst.data(), cids.data(), cw.data(), m, d_x, report, s); if (r) return r;
+        c->deformed.assign(c->slices.size(), kt_ctx::Deformed());
+        for (size_t i = 0; i < c->slices.size(); ++i) { c->deformed[i].processed = c->slices[i].processed; c->deformed[i].mesh_verts = c->slices[i].mesh_verts; }
+        if (!report->deformed) return 0;                                                  // the map as recorded
+        if (!c->deform_arena) c->deform_arena = new PinnedArena();
+        c->deform_arena->rewind();
+        KT_CUDA(cudaMalloc(&d_out, nmax * sizeof(kt_point_xyzrgbnormal)));
+        // the map, one kind at a time: upload from the slices' pinned buffers, weights, apply, download into the deformation arena
+        for (int kind = 0; kind < 2; ++kind) {
+            const size_t total = kind == 0 ? np : nm, rec = kind == 0 ? sizeof(kt_point_xyzrgbnormal) : sizeof(kt_mesh_vertex);
+            if (!total) continue;
+            std::vector<uint64_t> vt(total);
+            size_t off = 0;
+            for (const auto& sl : c->slices) {
+                const size_t cnt = kind == 0 ? (sl.has_processed ? sl.processed_count : 0) : (sl.has_mesh ? sl.mesh_nv : 0);
+                if (!cnt) continue;
+                KT_CUDA(cudaMemcpyAsync((char*)d_in + off * rec, kind == 0 ? (const void*)sl.processed : (const void*)sl.mesh_verts, cnt * rec, cudaMemcpyHostToDevice, s));
+                std::fill(vt.begin() + off, vt.begin() + off + cnt, sl.utime);             // a vertex's time is its slice's
+                off += cnt;
+            }
+            KT_CUDA(cudaMemcpyAsync(d_t, vt.data(), total * sizeof(uint64_t), cudaMemcpyHostToDevice, s));
+            r = deform_weights(d_npos, d_ntime, nn, d_in, kind, d_t, total, d_ids, d_w, s); if (r) return r;
+            r = deform_apply(d_npos, d_x, nn, d_ids, d_w, d_in, d_out, kind, total, s); if (r) return r;
+            off = 0;
+            for (size_t i = 0; i < c->slices.size(); ++i) {
+                const auto& sl = c->slices[i];
+                const size_t cnt = kind == 0 ? (sl.has_processed ? sl.processed_count : 0) : (sl.has_mesh ? sl.mesh_nv : 0);
+                if (!cnt) continue;
+                void* h = c->deform_arena->alloc(cnt * rec);
+                if (!h) { set_error("kt_deform_map: pinned host memory for %zu deformed records", cnt); return KT_ERR_CUDA; }
+                KT_CUDA(cudaMemcpyAsync(h, (const char*)d_out + off * rec, cnt * rec, cudaMemcpyDeviceToHost, s));
+                if (kind == 0) c->deformed[i].processed = (kt_point_xyzrgbnormal*)h; else c->deformed[i].mesh_verts = (kt_mesh_vertex*)h;
+                off += cnt;
+            }
+            KT_CUDA(cudaStreamSynchronize(s));                                            // vt and the device buffers are reused
+        }
+        return 0;
+    };
+    const int r = run();
+    cudaStreamSynchronize(c->stream);
+    cleanup();
+    if (r) c->deformed.clear();
+    return r;
+}
+
+int kt_get_deformed_slice(kt_ctx* c, int idx, kt_point_xyzrgbnormal* points, size_t max_points, size_t* count)
+{
+    if (!c || idx < 0 || idx >= (int)c->slices.size()) { set_error("kt_get_deformed_slice: bad index"); return KT_ERR_INVALID; }
+    if (idx >= (int)c->deformed.size()) { set_error("kt_get_deformed_slice: slice %d was recorded after the last kt_deform_map", idx); return KT_ERR_STATE; }
+    const SliceRec& s = c->slices[idx];
+    if (!s.has_processed) { set_error("kt_get_deformed_slice: slice %d was recorded with slice processing off (kt_set_slice_processing)", idx); return KT_ERR_STATE; }
+    if (count) *count = s.processed_count;
+    const size_t n = std::min(max_points, s.processed_count);
+    if (points && n) std::memcpy(points, c->deformed[idx].processed, n * sizeof(kt_point_xyzrgbnormal));
+    return KT_OK;
+}
+
+int kt_get_deformed_slice_mesh(kt_ctx* c, int idx, kt_mesh_vertex* verts, size_t max_verts, size_t* n_verts)
+{
+    if (!c || idx < 0 || idx >= (int)c->slices.size()) { set_error("kt_get_deformed_slice_mesh: bad index"); return KT_ERR_INVALID; }
+    if (idx >= (int)c->deformed.size()) { set_error("kt_get_deformed_slice_mesh: slice %d was recorded after the last kt_deform_map", idx); return KT_ERR_STATE; }
+    const SliceRec& s = c->slices[idx];
+    if (!s.has_mesh) { set_error("kt_get_deformed_slice_mesh: slice %d was recorded with meshing off (kt_set_slice_meshing)", idx); return KT_ERR_STATE; }
+    if (n_verts) *n_verts = s.mesh_nv;
+    const size_t n = std::min(max_verts, s.mesh_nv);
+    if (verts && n) std::memcpy(verts, c->deformed[idx].mesh_verts, n * sizeof(kt_mesh_vertex));
+    return KT_OK;
+}
+
+int kt_save_deformed_mesh_ply(kt_ctx* c, const char* path)
+{
+    if (!c || !path) return KT_ERR_INVALID;
+    if (c->deformed.empty()) { set_error("kt_save_deformed_mesh_ply: no kt_deform_map since the last reset"); return KT_ERR_STATE; }
+    return save_mesh_ply(c, path, c->deformed.size(), true, "kt_save_deformed_mesh_ply");
 }
 
 int kt_get_slice_info(kt_ctx* c, int idx, kt_slice_info* info)
