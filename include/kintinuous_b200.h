@@ -200,6 +200,47 @@ KT_API int kt_get_deformed_slice_mesh(kt_ctx* ctx, int idx, kt_mesh_vertex* vert
 /* The "_opt" mesh of Deformation::saveMesh (Deformation.cpp:85-100): kt_save_mesh_ply's layout over the deformed vertices of the slices
  * covered by the last kt_deform_map.  KT_ERR_STATE before any kt_deform_map or when none of those slices has a mesh. */
 KT_API int kt_save_deformed_mesh_ply(kt_ctx* ctx, const char* path);
+/* Loop closure: the pose-graph half of the reference's backend (backend/Deformation.cpp:130-346 addCameraCamera / addCameraLoop,
+ * backend/iSAMInterface.cpp) on the GPU.  The caller passes what PlaceRecognition produces (LoopClosureConstraint,
+ * PlaceRecognition.cpp:198-209): time1 (the new frame) and time2 (the old one), both dense pose timestamps, the pose of the camera at
+ * time2 in the frame of the camera at time1 (row-major 4 x 4, ~ P(time1)^-1 P(time2)) and the PnP inliers seen from each camera
+ * (camera-frame xyz, n_inliers of each).  Loop detection itself stays with the caller.
+ *   - Nodes: every dense pose (pose_spacing 0), or the first, each more than pose_spacing from the last taken (the reference's -fl with
+ *     -dg), and every pose a loop names; the last dense pose always.  Odometry factors join consecutive nodes; one factor per loop; a
+ *     prior anchors the first node at its tracked pose; covariance 1e-3 I everywhere (iSAMInterface.cpp:44-105).
+ *   - Every call re-optimises the whole graph from the tracked trajectory with every accepted loop plus the new one (FP64 Gauss-Newton,
+ *     at most 100 steps, until chi2 falls by less than 1e-3 or 1e-5 relative).  chi2 < isam_thresh (the reference's -it, 10) accepts
+ *     the loop; otherwise nothing observable changes (Deformation.cpp:254-343).
+ *   - On acceptance the map recorded so far (as kt_deform_map, node_spacing its -dg) is deformed from the original slices: each node's
+ *     tracked position to its optimised one, and each inlier of every accepted loop from its tracked to its optimised position.
+ *     Without processed slices or meshes only the trajectory is corrected (map_deformed = 0).
+ * Every check comes first and a failed one changes nothing: times in the dense pose graph (KT_ERR_INVALID), time1 != time2, finite input,
+ * a rotation within 1e-3 of orthonormal, enough deformation nodes for a recorded map (KT_ERR_STATE), at most 64 accepted loops
+ * (KT_ERR_CAPACITY).  A CUDA error while the map is deformed drops the deformed copies (as kt_deform_map) and does not record the loop.
+ * Tracking never reads the corrected poses.  A volume shared by several GPUs: KT_ERR_INVALID. */
+typedef struct kt_loop_constraint {
+    uint64_t time1, time2;
+    double constraint[16];
+    const float* inliers1;          /* n_inliers xyz triples in the camera at time1 (inliers1Proj); may be NULL when n_inliers == 0 */
+    const float* inliers2;          /* n_inliers xyz triples in the camera at time2 (inliers2Proj) */
+    size_t n_inliers;
+} kt_loop_constraint;
+typedef struct kt_loop_report {
+    int nodes, factors, loops, iterations;
+    double chi2_initial, chi2_final;    /* sum of squared whitened errors before / after the optimisation */
+    int accepted;                       /* chi2_final < isam_thresh and the factorisation succeeded */
+    int solver_failed;                  /* a pivot was not positive: the loop is rejected */
+    int map_deformed;                   /* the deformation moved the map (deform.deformed); deform holds that run's report, which is
+                                           all zero when no map is recorded or the loop is rejected */
+    kt_deform_report deform;
+} kt_loop_report;
+KT_API int kt_close_loop(kt_ctx* ctx, const kt_loop_constraint* loop, float pose_spacing, float node_spacing, double isam_thresh,
+                         kt_loop_report* report);
+KT_API int kt_num_loops(kt_ctx* ctx);                                      /* accepted loops since the last reset */
+/* The optimised nodes of the last accepted loop (timestamp, world-frame pose, is_loop_pose = named by a loop): the corrected
+ * trajectory (iSAMInterface::getCameraPoses, :169-182).  0 nodes before any accepted loop. */
+KT_API int kt_num_pose_graph_nodes(kt_ctx* ctx);
+KT_API int kt_get_pose_graph_node(kt_ctx* ctx, int idx, kt_dense_pose* out);
 /* KintinuousTracker::outputPose (.cpp:199-218, :911-914): append one line per tracked frame to `path` ("<saveFile>.poses" in the
  * reference: "utime/1e6 gx gy gz qx qy qz qw").  NULL closes the log.  kt_format_pose_line formats one such line into buf. */
 KT_API int kt_set_pose_log(kt_ctx* ctx, const char* path);
@@ -345,6 +386,20 @@ KT_API int kt_op_deform_optimise(const float* node_pos_dev, int n_nodes, const f
  * other byte copied. */
 KT_API int kt_op_deform_apply(const float* node_pos_dev, const double* params_dev, int n_nodes, const int32_t* ids_dev,
                               const double* weights_dev, const void* in_dev, void* out_dev, int kind, size_t n, void* stream);
+/* Pose-graph optimisation (isam::Slam::batch_optimization as kt_close_loop runs it).  poses_dev: n_nodes 4 x 4 row-major FP64 node
+ * poses, the initial estimate; factors_dev: n_factors kt_pgo_factor records -- factor 0 the prior on node 0 (i = -1, z = the anchor's
+ * Pose3d vector x y z yaw pitch roll), factor k (1 <= k < n_nodes) odometry k-1 -> k, then at most 64 loops (any i != j); z of a
+ * between factor is the measured (p_j (-) p_i).vector().  out_dev: the optimised poses (may equal poses_dev).  Any other list shape:
+ * KT_ERR_INVALID; more than 2^18 nodes or 64 loops: KT_ERR_CAPACITY. */
+typedef struct kt_pgo_factor { int32_t i, j; double z[6]; } kt_pgo_factor;
+typedef struct kt_pgo_report {
+    int nodes, factors, loops, iterations;
+    double chi2_initial, chi2_final;
+    int solver_failed;
+    double step_ms;                 /* mean device time of a Gauss-Newton step (assembly to the chi2 of the updated poses), CUDA events */
+} kt_pgo_report;
+KT_API int kt_op_pgo_optimise(const double* poses_dev, int n_nodes, const kt_pgo_factor* factors_dev, int n_factors, double* out_dev,
+                              kt_pgo_report* report, void* stream);
 /* clearVolume{X,Y,Z}[Back] + ...c on both volumes (tsdf_volume.cu:117-448). axis 0..2, back 0/1. */
 KT_API int kt_op_clear_volume(int axis, int back, int16_t* tsdf_dev, uint8_t* color_dev, int vol, int current_wrap, int delta_wrap, void* stream);
 /* initVolume + initColorVolume (tsdf_volume.cu:469, :77) */

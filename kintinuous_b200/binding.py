@@ -85,6 +85,38 @@ class DeformReport(C.Structure):
         return {k: getattr(self, k) for k, _ in self._fields_}
 
 
+class LoopConstraint(C.Structure):
+    """kt_loop_constraint: PlaceRecognition's LoopClosureConstraint (time1 new, time2 old, pose of time2 in time1's camera, inliers)."""
+    _fields_ = [("time1", C.c_uint64), ("time2", C.c_uint64), ("constraint", C.c_double * 16), ("inliers1", C.c_void_p),
+                ("inliers2", C.c_void_p), ("n_inliers", C.c_size_t)]
+
+
+class LoopReport(C.Structure):
+    """kt_loop_report of kt_close_loop."""
+    _fields_ = [("nodes", C.c_int), ("factors", C.c_int), ("loops", C.c_int), ("iterations", C.c_int),
+                ("chi2_initial", C.c_double), ("chi2_final", C.c_double), ("accepted", C.c_int), ("solver_failed", C.c_int),
+                ("map_deformed", C.c_int), ("deform", DeformReport)]
+
+    def as_dict(self):
+        d = {k: getattr(self, k) for k, _ in self._fields_ if k != "deform"}
+        d["deform"] = self.deform.as_dict()
+        return d
+
+
+class PgoReport(C.Structure):
+    """kt_pgo_report of kt_op_pgo_optimise."""
+    _fields_ = [("nodes", C.c_int), ("factors", C.c_int), ("loops", C.c_int), ("iterations", C.c_int),
+                ("chi2_initial", C.c_double), ("chi2_final", C.c_double), ("solver_failed", C.c_int), ("step_ms", C.c_double)]
+
+    def as_dict(self):
+        return {k: getattr(self, k) for k, _ in self._fields_}
+
+
+# kt_pgo_factor (56 bytes): i = -1 for the prior on node j
+PGO_FACTOR_DTYPE = np.dtype([("i", "<i4"), ("j", "<i4"), ("z", "<f8", (6,))])
+assert PGO_FACTOR_DTYPE.itemsize == 56
+
+
 class SliceInfo(C.Structure):
     _fields_ = [("dimension", C.c_int), ("odometry", C.c_int), ("camera_t", C.c_float * 3), ("camera_R", C.c_float * 9),
                 ("utime", C.c_uint64), ("count", C.c_size_t)]
@@ -278,6 +310,32 @@ class Tracker:
     def save_deformed_mesh_ply(self, path):
         """The deformed slice meshes of the last deform_map as one binary PLY (kt_save_deformed_mesh_ply)."""
         _check(self.lib.kt_save_deformed_mesh_ply(self.h, os.fsencode(path)))
+
+    def close_loop(self, time1, time2, T, inliers1=None, inliers2=None, pose_spacing=0.0, node_spacing=0.8, isam_thresh=10.0):
+        """Close a loop (kt_close_loop): T = pose of the camera at time2 in the frame of the camera at time1 (4 x 4); inliers1 / inliers2:
+        [n, 3] camera-frame points seen at time1 / time2.  Returns the LoopReport (accepted, chi2, the map deformation)."""
+        lc = LoopConstraint(time1=int(time1), time2=int(time2))
+        lc.constraint[:] = [float(v) for v in np.asarray(T, np.float64).reshape(16)]
+        a = np.ascontiguousarray(np.asarray(inliers1 if inliers1 is not None else np.zeros((0, 3)), np.float32).reshape(-1, 3))
+        b = np.ascontiguousarray(np.asarray(inliers2 if inliers2 is not None else np.zeros((0, 3)), np.float32).reshape(-1, 3))
+        if len(a) != len(b):
+            raise ValueError("inliers1 and inliers2 must have the same length")
+        lc.inliers1 = a.ctypes.data if len(a) else None; lc.inliers2 = b.ctypes.data if len(b) else None; lc.n_inliers = len(a)
+        rep = LoopReport()
+        _check(self.lib.kt_close_loop(self.h, C.byref(lc), C.c_float(pose_spacing), C.c_float(node_spacing), C.c_double(isam_thresh), C.byref(rep)))
+        return rep
+
+    def num_loops(self):
+        return int(self.lib.kt_num_loops(self.h))
+
+    def pose_graph_nodes(self):
+        """[(timestamp, 4x4 world-frame pose, is_loop_pose)] of the last accepted loop's optimised pose graph (empty before one)."""
+        out = []
+        for i in range(int(self.lib.kt_num_pose_graph_nodes(self.h))):
+            d = DensePose()
+            _check(self.lib.kt_get_pose_graph_node(self.h, i, C.byref(d)))
+            out.append((int(d.timestamp), np.array(d.pose, np.float32).reshape(4, 4), bool(d.is_loop_pose)))
+        return out
 
     def slice_info(self, idx):
         """The rest of the CloudSlice record: dimension, odometry kind, camera pose at hand-over, timestamp, point count."""
@@ -514,6 +572,15 @@ class _Ops:
         """kt_op_deform_apply: n records of kind 0 (POINT_NORMAL) / 1 (MESH_VERTEX) from points_in to points_out."""
         _check(self._l().kt_op_deform_apply(_ptr(node_pos), _ptr(params), int(node_pos.shape[0]), _ptr(ids), _ptr(weights), _ptr(points_in),
                                             _ptr(points_out), int(kind), C.c_size_t(int(n)), None))
+
+    def pgo_optimise(self, poses, factors, out):
+        """kt_op_pgo_optimise: poses float64 [n, 4, 4] (device), factors PGO_FACTOR_DTYPE records as a device byte tensor; writes the
+        optimised poses to out (may be poses).  Returns the PgoReport."""
+        rep = PgoReport()
+        n = int(poses.numel() // 16)
+        _check(self._l().kt_op_pgo_optimise(_ptr(poses), n, _ptr(factors), int(factors.numel() // PGO_FACTOR_DTYPE.itemsize), _ptr(out),
+                                            C.byref(rep), None))
+        return rep
 
     def clear_volume(self, axis, back, tsdf, color, vol, current, delta):
         _check(self._l().kt_op_clear_volume(axis, back, _ptr(tsdf), _ptr(color), vol, current, delta, None))

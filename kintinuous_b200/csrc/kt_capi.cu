@@ -2,6 +2,7 @@
 // src/frontend/cuda/internal.h:299-536, same argument meaning, synchronous semantics (results visible on return),
 // status codes instead of exit(0).  The tracker-level ABI (kt_create / kt_process_frame / ...) is in kt_tracker.cu.
 #include "kt_ops.h"
+#include "kt_pgo.hpp"
 #include "../../include/kintinuous_b200.h"
 #include <cstring>
 #include <cstddef>
@@ -233,6 +234,17 @@ int kt_op_deform_optimise(const float* node_pos, int n_nodes, const float* con_s
     }
     KT_CUDA(cudaStreamSynchronize(st(s)));
     return deform_optimise(pos.data(), n_nodes, src.data(), dst.data(), ids.data(), w.data(), m, params, report, st(s));
+}
+
+// isam::Slam::batch_optimization (iSAMInterface.cpp:136-140) over a caller's graph
+int kt_op_pgo_optimise(const double* poses, int n_nodes, const kt_pgo_factor* factors, int n_factors, double* out, kt_pgo_report* report, void* s)
+{
+    static_assert(sizeof(kt_pgo_factor) == sizeof(PgoFactor) && offsetof(kt_pgo_factor, z) == offsetof(PgoFactor, z), "kt_pgo_factor layout");
+    if (!poses || !factors || !out || !report || n_nodes < 2 || n_factors < n_nodes) { set_error("kt_op_pgo_optimise: bad argument"); return KT_ERR_INVALID; }
+    std::vector<PgoFactor> f(n_factors);
+    KT_CUDA(cudaMemcpyAsync(f.data(), factors, f.size() * sizeof(PgoFactor), cudaMemcpyDeviceToHost, st(s)));
+    KT_CUDA(cudaStreamSynchronize(st(s)));
+    return pgo_optimise(poses, n_nodes, f.data(), n_factors, out, report, st(s));
 }
 
 int kt_op_deform_apply(const float* node_pos, const double* params, int n_nodes, const int32_t* ids, const double* weights, const void* in,

@@ -4,6 +4,7 @@
 #include "kt_common.cuh"
 
 struct kt_deform_report;
+struct kt_pgo_report;
 
 namespace kt {
 
@@ -199,6 +200,11 @@ int deform_optimise(const float* node_pos, int n_nodes, const float* src, const 
 // Deforms n records of kind 0 / 1 from in to out (may not alias) with the nodes' unknowns x; asynchronous.
 int deform_apply(const float* node_pos, const double* x, int n_nodes, const int32_t* ids, const double* weights, const void* in, void* out,
                  int kind, size_t n, cudaStream_t s);
+// ---- pose-graph optimisation (kt_pgo.cu, host logic in kt_pgo.hpp) ----
+struct PgoFactor;
+// Gauss-Newton from poses_in (device, n x 16 FP64) into X (device, may alias) over the host factor list; every field of the report.
+// Synchronises s.
+int pgo_optimise(const double* poses_in, int n, const PgoFactor* factors, int n_factors, double* X, kt_pgo_report* rep, cudaStream_t s);
 // cross-GPU barrier: every rank writes `epoch` into slot [rank] of every peer's flag array, then waits until all slots of its own
 // array reach `epoch` (bounded spin: returns through *error_dev != 0 instead of hanging the GPU if a peer never arrives)
 int xgpu_barrier(unsigned int* const* peer_flags_dev /* [world] device array of pointers */, unsigned int* my_flags, int rank, int world,

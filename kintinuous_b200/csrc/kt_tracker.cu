@@ -16,9 +16,11 @@
 #include "kt_shift.hpp"
 #include "kt_posegraph.hpp"
 #include "kt_deform.hpp"
+#include "kt_pgo.hpp"
 #include <cstdlib>
 #include "../../include/kintinuous_b200.h"
 #include <vector>
+#include <unordered_map>
 #include <cstring>
 #include <cmath>
 #include <climits>
@@ -161,6 +163,9 @@ struct kt_ctx {
     // arena, or the slice's own buffers when the call left the map unchanged
     struct Deformed { kt_point_xyzrgbnormal* processed; kt_mesh_vertex* mesh_verts; };
     std::vector<Deformed> deformed; PinnedArena* deform_arena;
+    // loop closure (kt_close_loop, kt_pgo.cu): the accepted loops with their inliers, and the optimised nodes of the last accepted one
+    struct Loop { uint64_t time1, time2; double C[16]; std::vector<float> in1, in2; };
+    std::vector<Loop> loops; std::vector<kt_dense_pose> pgo_nodes;
     // RGB-D
     float* lastDepth[LEVELS]; float* nextDepth[LEVELS]; uint8_t* lastImage[LEVELS]; uint8_t* nextImage[LEVELS];
     int16_t* nextdIdx[LEVELS]; int16_t* nextdIdy[LEVELS]; float* pointClouds[LEVELS]; void* corresImg[LEVELS];
@@ -649,6 +654,7 @@ int kt_reset(kt_ctx* c)
     drop_slices(c);
     c->deformed.clear();
     if (c->deform_arena) c->deform_arena->rewind();
+    c->loops.clear(); c->pgo_nodes.clear();
     c->dense_poses.clear();                      // reset(): densePoseGraph.clear(), latestDensePoseId = 0 (.cpp:300-301)
     c->trace_iters = 0; c->shifted_last = 0; c->cloud_count = 0;
     c->pf_valid = false; c->pf_built = false; c->frontend_ready = false; c->maps_on_stream = false;
@@ -1102,59 +1108,44 @@ int kt_save_mesh_ply(kt_ctx* c, const char* path)
     return save_mesh_ply(c, path, c->slices.size(), false, "kt_save_mesh_ply");
 }
 
-// Deformation::addCameraLoop's graph work (Deformation.cpp:264-318: appendVertices, the camera-pose constraints, optimiseGraphSparse,
-// applyGraphToVertices) over the map recorded so far, on the tracker's stream.  Nothing the tracker reads is written.
-int kt_deform_map(kt_ctx* c, const kt_dense_pose* corrected, size_t n, const kt_deform_constraint* points, size_t n_points, float node_spacing,
-                  kt_deform_report* report)
+// The deformation graph's nodes (initialiseGraphPoses): the dense pose graph's positions, the first and every one more than node_spacing
+// from the last taken.  KT_ERR_STATE without a recorded map, with fewer than k + 1 nodes or with descending timestamps.
+static int deform_nodes(kt_ctx* c, float node_spacing, std::vector<float>& npos, std::vector<uint64_t>& ntime, const char* who)
 {
-    if (!c || !report || (n && !corrected) || (n_points && !points) || !(node_spacing >= 0.f)) { set_error("kt_deform_map: bad argument"); return KT_ERR_INVALID; }
-    std::memset(report, 0, sizeof(*report));
-    if (c->world > 1) { set_error("kt_deform_map: a volume shared by %d GPUs cannot be deformed", c->world); return KT_ERR_INVALID; }
-    size_t np = 0, nm = 0; bool any = false;
-    for (const auto& s : c->slices) {
-        if (s.has_processed) { any = true; np += s.processed_count; }
-        if (s.has_mesh) { any = true; nm += s.mesh_nv; }
-    }
-    if (!any) { set_error("kt_deform_map: no processed slice and no slice mesh recorded (kt_set_slice_processing / kt_set_slice_meshing)"); return KT_ERR_STATE; }
-    // nodes: the dense pose graph's positions (initialiseGraphPoses)
+    bool any = false;
+    for (const auto& s : c->slices) if (s.has_processed || s.has_mesh) any = true;
+    if (!any) { set_error("%s: no processed slice and no slice mesh recorded (kt_set_slice_processing / kt_set_slice_meshing)", who); return KT_ERR_STATE; }
     const size_t nd = c->dense_poses.size();
-    std::vector<float> gpos(nd * 3); std::vector<uint64_t> gtime(nd);
-    for (size_t i = 0; i < nd; ++i) {
-        gtime[i] = c->dense_poses[i].timestamp;
-        for (int e = 0; e < 3; ++e) gpos[3 * i + e] = c->dense_poses[i].pose[4 * e + 3];
-    }
+    std::vector<float> gpos(nd * 3);
+    for (size_t i = 0; i < nd; ++i) for (int e = 0; e < 3; ++e) gpos[3 * i + e] = c->dense_poses[i].pose[4 * e + 3];
     const std::vector<int> take = deform_sample_nodes(gpos.data(), nd, node_spacing);
     const int nn = (int)take.size();
     if (nn < DEFORM_K + 1) {
-        set_error("kt_deform_map: node_spacing %g m leaves %d graph nodes on the trajectory; at least %d are needed", (double)node_spacing, nn, DEFORM_K + 1);
+        set_error("%s: node_spacing %g m leaves %d graph nodes on the trajectory; at least %d are needed", who, (double)node_spacing, nn, DEFORM_K + 1);
         return KT_ERR_STATE;
     }
-    std::vector<float> npos(3 * (size_t)nn); std::vector<uint64_t> ntime(nn);
-    for (int j = 0; j < nn; ++j) { ntime[j] = gtime[take[j]]; for (int e = 0; e < 3; ++e) npos[3 * j + e] = gpos[3 * take[j] + e]; }
+    npos.resize(3 * (size_t)nn); ntime.resize(nn);
+    for (int j = 0; j < nn; ++j) { ntime[j] = c->dense_poses[take[j]].timestamp; for (int e = 0; e < 3; ++e) npos[3 * j + e] = gpos[3 * take[j] + e]; }
     for (int j = 1; j < nn; ++j)
-        if (ntime[j] < ntime[j - 1]) { set_error("kt_deform_map: the dense pose graph's timestamps are not ascending"); return KT_ERR_STATE; }
-    // constraints: corrected camera positions, then the caller's points
-    std::vector<uint64_t> ctime(n); std::vector<double> cpos(3 * n);
-    for (size_t i = 0; i < n; ++i) { ctime[i] = corrected[i].timestamp; for (int e = 0; e < 3; ++e) cpos[3 * i + e] = corrected[i].pose[4 * e + 3]; }
-    std::vector<DeformConstraint> cons;
-    const long miss = deform_pose_constraints(gtime.data(), gpos.data(), nd, ctime.data(), cpos.data(), n, cons);
-    if (miss >= 0) { set_error("kt_deform_map: corrected pose %ld has timestamp %llu, which is not in the dense pose graph", miss, (unsigned long long)ctime[miss]); return KT_ERR_INVALID; }
-    for (size_t i = 0; i < n_points; ++i) {
-        DeformConstraint q; q.time = points[i].time;
-        for (int e = 0; e < 3; ++e) { q.src[e] = points[i].source[e]; q.dst[e] = points[i].target[e]; }
-        cons.push_back(q);
+        if (ntime[j] < ntime[j - 1]) { set_error("%s: the dense pose graph's timestamps are not ascending", who); return KT_ERR_STATE; }
+    return 0;
+}
+
+// Deformation::addCameraLoop's graph work (Deformation.cpp:264-318: appendVertices, the constraints, optimiseGraphSparse,
+// applyGraphToVertices) over the map recorded so far, on the tracker's stream, with checked, finite constraints.  Nothing the tracker
+// reads is written; c->deformed holds the result (cleared on an error).
+static int deform_run(kt_ctx* c, const std::vector<float>& npos, const std::vector<uint64_t>& ntime, const std::vector<DeformConstraint>& cons,
+                      kt_deform_report* report)
+{
+    const int nn = (int)ntime.size();
+    size_t np = 0, nm = 0;
+    for (const auto& s : c->slices) {
+        if (s.has_processed) np += s.processed_count;
+        if (s.has_mesh) nm += s.mesh_nv;
     }
     const size_t m = cons.size();
-    if (!m) { set_error("kt_deform_map: no constraints"); return KT_ERR_INVALID; }
-    for (size_t l = 0; l < m; ++l)
-        if (deform_first_non_finite(cons[l].src, 3) >= 0 || deform_first_non_finite(cons[l].dst, 3) >= 0) {
-            if (l < n) set_error("kt_deform_map: corrected pose %zu has a translation that is not finite", l);
-            else set_error("kt_deform_map: point constraint %zu has a source or target that is not finite", l - n);
-            return KT_ERR_INVALID;
-        }
     std::vector<float> csrc(3 * m); std::vector<double> cdst(3 * m); std::vector<uint64_t> ct(m);
     for (size_t l = 0; l < m; ++l) { ct[l] = cons[l].time; for (int e = 0; e < 3; ++e) { csrc[3 * l + e] = cons[l].src[e]; cdst[3 * l + e] = cons[l].dst[e]; } }
-
     KT_CUDA(cudaSetDevice(c->cfg.device));
     if (c->stream_slices) KT_CUDA(cudaStreamSynchronize(c->stream_slices));           // every slice has landed in its pinned buffers
     const size_t nmax = std::max(std::max(np, nm), m);
@@ -1222,6 +1213,162 @@ int kt_deform_map(kt_ctx* c, const kt_dense_pose* corrected, size_t n, const kt_
     cleanup();
     if (r) c->deformed.clear();
     return r;
+}
+
+
+int kt_deform_map(kt_ctx* c, const kt_dense_pose* corrected, size_t n, const kt_deform_constraint* points, size_t n_points, float node_spacing,
+                  kt_deform_report* report)
+{
+    if (!c || !report || (n && !corrected) || (n_points && !points) || !(node_spacing >= 0.f)) { set_error("kt_deform_map: bad argument"); return KT_ERR_INVALID; }
+    std::memset(report, 0, sizeof(*report));
+    if (c->world > 1) { set_error("kt_deform_map: a volume shared by %d GPUs cannot be deformed", c->world); return KT_ERR_INVALID; }
+    std::vector<float> npos; std::vector<uint64_t> ntime;
+    int r = deform_nodes(c, node_spacing, npos, ntime, "kt_deform_map"); if (r) return r;
+    // constraints: corrected camera positions, then the caller's points
+    const size_t nd = c->dense_poses.size();
+    std::vector<float> gpos(nd * 3); std::vector<uint64_t> gtime(nd);
+    for (size_t i = 0; i < nd; ++i) { gtime[i] = c->dense_poses[i].timestamp; for (int e = 0; e < 3; ++e) gpos[3 * i + e] = c->dense_poses[i].pose[4 * e + 3]; }
+    std::vector<uint64_t> ctime(n); std::vector<double> cpos(3 * n);
+    for (size_t i = 0; i < n; ++i) { ctime[i] = corrected[i].timestamp; for (int e = 0; e < 3; ++e) cpos[3 * i + e] = corrected[i].pose[4 * e + 3]; }
+    std::vector<DeformConstraint> cons;
+    const long miss = deform_pose_constraints(gtime.data(), gpos.data(), nd, ctime.data(), cpos.data(), n, cons);
+    if (miss >= 0) { set_error("kt_deform_map: corrected pose %ld has timestamp %llu, which is not in the dense pose graph", miss, (unsigned long long)ctime[miss]); return KT_ERR_INVALID; }
+    for (size_t i = 0; i < n_points; ++i) {
+        DeformConstraint q; q.time = points[i].time;
+        for (int e = 0; e < 3; ++e) { q.src[e] = points[i].source[e]; q.dst[e] = points[i].target[e]; }
+        cons.push_back(q);
+    }
+    const size_t m = cons.size();
+    if (!m) { set_error("kt_deform_map: no constraints"); return KT_ERR_INVALID; }
+    for (size_t l = 0; l < m; ++l)
+        if (deform_first_non_finite(cons[l].src, 3) >= 0 || deform_first_non_finite(cons[l].dst, 3) >= 0) {
+            if (l < n) set_error("kt_deform_map: corrected pose %zu has a translation that is not finite", l);
+            else set_error("kt_deform_map: point constraint %zu has a source or target that is not finite", l - n);
+            return KT_ERR_INVALID;
+        }
+    return deform_run(c, npos, ntime, cons, report);
+}
+
+// Deformation::addCameraCamera + addCameraLoop (Deformation.cpp:130-346) with iSAMInterface (iSAMInterface.cpp:44-140): the pose graph of
+// the dense poses, every accepted loop and the new one, optimised from the tracked trajectory on the GPU (kt_pgo.cu); the chi2 gate; on
+// acceptance the map deformation of kt_deform_map.  Every check precedes any change of state.
+int kt_close_loop(kt_ctx* c, const kt_loop_constraint* loop, float pose_spacing, float node_spacing, double isam_thresh, kt_loop_report* report)
+{
+    if (!c || !loop || !report || !(pose_spacing >= 0.f) || !(node_spacing >= 0.f) || !(isam_thresh > 0.0) ||
+        (loop->n_inliers && (!loop->inliers1 || !loop->inliers2))) { set_error("kt_close_loop: bad argument"); return KT_ERR_INVALID; }
+    std::memset(report, 0, sizeof(*report));
+    if (c->world > 1) { set_error("kt_close_loop: a volume shared by %d GPUs cannot be loop-closed", c->world); return KT_ERR_INVALID; }
+    if (c->loops.size() >= (size_t)PGO_MAX_LOOPS) { set_error("kt_close_loop: %zu loops accepted already, at most %d", c->loops.size(), PGO_MAX_LOOPS); return KT_ERR_CAPACITY; }
+    if (loop->time1 == loop->time2) { set_error("kt_close_loop: time1 == time2"); return KT_ERR_INVALID; }
+    const int chk = pgo_check_constraint(loop->constraint);
+    if (chk) { set_error(chk == 1 ? "kt_close_loop: the constraint is not finite" : "kt_close_loop: the constraint's rotation is not orthonormal within 1e-3"); return KT_ERR_INVALID; }
+    if (deform_first_non_finite(loop->inliers1, 3 * loop->n_inliers) >= 0 || deform_first_non_finite(loop->inliers2, 3 * loop->n_inliers) >= 0) {
+        set_error("kt_close_loop: an inlier is not finite"); return KT_ERR_INVALID;
+    }
+    const size_t nd = c->dense_poses.size();
+    std::unordered_map<uint64_t, int> at;                         // the last dense pose with a timestamp (iSAM's std::map cameraNode)
+    for (size_t i = 0; i < nd; ++i) at[c->dense_poses[i].timestamp] = (int)i;
+    if (!at.count(loop->time1) || !at.count(loop->time2)) { set_error("kt_close_loop: time %llu is not in the dense pose graph",
+        (unsigned long long)(at.count(loop->time1) ? loop->time2 : loop->time1)); return KT_ERR_INVALID; }
+    bool map = false;
+    for (const auto& sl : c->slices) if (sl.has_processed || sl.has_mesh) map = true;
+    std::vector<float> npos; std::vector<uint64_t> ntime;
+    if (map) { const int r = deform_nodes(c, node_spacing, npos, ntime, "kt_close_loop"); if (r) return r; }
+
+    // the loops: accepted ones, then the new one
+    std::vector<kt_ctx::Loop> loops = c->loops;
+    { kt_ctx::Loop l; l.time1 = loop->time1; l.time2 = loop->time2; std::memcpy(l.C, loop->constraint, sizeof(l.C));
+      l.in1.assign(loop->inliers1, loop->inliers1 + 3 * loop->n_inliers); l.in2.assign(loop->inliers2, loop->inliers2 + 3 * loop->n_inliers);
+      loops.push_back(l); }
+    // nodes (addCameraCamera)
+    std::vector<float> gpos(nd * 3); std::vector<unsigned char> flagged(nd, 0);
+    for (size_t i = 0; i < nd; ++i) { flagged[i] = c->dense_poses[i].is_loop_pose ? 1 : 0; for (int e = 0; e < 3; ++e) gpos[3 * i + e] = c->dense_poses[i].pose[4 * e + 3]; }
+    for (const auto& l : loops) { flagged[at[l.time1]] = 1; flagged[at[l.time2]] = 1; }
+    const std::vector<int> take = pgo_select_nodes(gpos.data(), flagged.data(), nd, pose_spacing);
+    const int n = (int)take.size();
+    if (n < 2) { set_error("kt_close_loop: the dense pose graph has %d poses", n); return KT_ERR_STATE; }
+    if (n > PGO_MAX_NODES) { set_error("kt_close_loop: %d pose-graph nodes, at most %d (raise pose_spacing)", n, PGO_MAX_NODES); return KT_ERR_CAPACITY; }
+    for (int k = 1; k < n; ++k)
+        if (c->dense_poses[take[k]].timestamp <= c->dense_poses[take[k - 1]].timestamp) { set_error("kt_close_loop: the dense pose graph's timestamps are not ascending"); return KT_ERR_STATE; }
+    std::unordered_map<int, int> node_of;
+    for (int k = 0; k < n; ++k) node_of[take[k]] = k;
+    // factors (cameraNode's prior, addCameraCameraConstraint, addLoopConstraint) and the initial estimate in the isam frame
+    std::vector<double> X0(16 * (size_t)n);
+    for (int k = 0; k < n; ++k) pgo_pose_to_isam(c->dense_poses[take[k]].pose, &X0[16 * (size_t)k]);
+    std::vector<PgoFactor> f(n + loops.size());
+    f[0].i = -1; f[0].j = 0; pgo_vector(&X0[0], f[0].z);
+    for (int k = 1; k < n; ++k) { f[k].i = k - 1; f[k].j = k; pgo_odometry_z(c->dense_poses[take[k - 1]].pose, c->dense_poses[take[k]].pose, f[k].z); }
+    for (size_t l = 0; l < loops.size(); ++l) {
+        PgoFactor& q = f[n + l];
+        q.i = node_of[at[loops[l].time1]]; q.j = node_of[at[loops[l].time2]];
+        pgo_loop_z(loops[l].C, q.z);
+    }
+
+    KT_CUDA(cudaSetDevice(c->cfg.device));
+    double* d_X = 0;
+    KT_CUDA(cudaMalloc((void**)&d_X, X0.size() * sizeof(double)));
+    std::vector<double> X(X0.size());
+    kt_pgo_report pr;
+    int r = 0;
+    if (!(r = kt::cuda_check(cudaMemcpyAsync(d_X, X0.data(), X0.size() * sizeof(double), cudaMemcpyHostToDevice, c->stream), "upload", __FILE__, __LINE__)))
+        r = pgo_optimise(d_X, n, f.data(), (int)f.size(), d_X, &pr, c->stream);
+    if (!r) r = kt::cuda_check(cudaMemcpy(X.data(), d_X, X.size() * sizeof(double), cudaMemcpyDeviceToHost), "download", __FILE__, __LINE__);
+    cudaFree(d_X);
+    if (r) return r;
+    report->nodes = pr.nodes; report->factors = pr.factors; report->loops = pr.loops; report->iterations = pr.iterations;
+    report->chi2_initial = pr.chi2_initial; report->chi2_final = pr.chi2_final; report->solver_failed = pr.solver_failed;
+    report->accepted = !pr.solver_failed && pr.chi2_final < isam_thresh;          // Deformation.cpp:256
+    if (!report->accepted) return KT_OK;                                            // :336-343: nothing observable changes
+
+    // the optimised nodes in the world frame
+    std::vector<kt_dense_pose> nodes(n);
+    std::vector<double> Pw(16 * (size_t)n);
+    for (int k = 0; k < n; ++k) {
+        pgo_pose_from_isam(&X[16 * (size_t)k], &Pw[16 * (size_t)k]);
+        nodes[k].timestamp = c->dense_poses[take[k]].timestamp; nodes[k].is_loop_pose = flagged[take[k]];
+        for (int q = 0; q < 16; ++q) nodes[k].pose[q] = (float)Pw[16 * (size_t)k + q];
+    }
+    if (map) {
+        // one position constraint per node, one point constraint per inlier of every accepted loop (addCameraLoop :192-315)
+        std::vector<DeformConstraint> cons;
+        for (int k = 0; k < n; ++k) {
+            DeformConstraint q; q.time = nodes[k].timestamp;
+            for (int e = 0; e < 3; ++e) { q.src[e] = c->dense_poses[take[k]].pose[4 * e + 3]; q.dst[e] = Pw[16 * (size_t)k + 4 * e + 3]; }
+            cons.push_back(q);
+        }
+        for (const auto& l : loops)
+            for (int side = 0; side < 2; ++side) {
+                const uint64_t t = side ? l.time2 : l.time1;
+                const std::vector<float>& in = side ? l.in2 : l.in1;
+                const float* Pt = c->dense_poses[at[t]].pose;
+                const double* Po = &Pw[16 * (size_t)node_of[at[t]]];
+                for (size_t p = 0; p + 2 < in.size(); p += 3) {
+                    DeformConstraint q; q.time = t;
+                    for (int e = 0; e < 3; ++e) {
+                        q.src[e] = (float)((double)Pt[4 * e] * in[p] + (double)Pt[4 * e + 1] * in[p + 1] + (double)Pt[4 * e + 2] * in[p + 2] + (double)Pt[4 * e + 3]);
+                        q.dst[e] = Po[4 * e] * in[p] + Po[4 * e + 1] * in[p + 1] + Po[4 * e + 2] * in[p + 2] + Po[4 * e + 3];
+                    }
+                    cons.push_back(q);
+                }
+            }
+        // A CUDA error here drops the deformed copies, as kt_deform_map does, and the loop is not recorded: the loops and the corrected
+        // trajectory stay those of the last accepted loop, and the next accepted loop deforms the original slices again.
+        r = deform_run(c, npos, ntime, cons, &report->deform);
+        if (r) return r;
+        report->map_deformed = report->deform.deformed;
+    }
+    c->loops.swap(loops);
+    c->pgo_nodes.swap(nodes);
+    return KT_OK;
+}
+
+int kt_num_loops(kt_ctx* c) { return c ? (int)c->loops.size() : 0; }
+int kt_num_pose_graph_nodes(kt_ctx* c) { return c ? (int)c->pgo_nodes.size() : 0; }
+int kt_get_pose_graph_node(kt_ctx* c, int idx, kt_dense_pose* out)
+{
+    if (!c || !out || idx < 0 || idx >= (int)c->pgo_nodes.size()) { set_error("kt_get_pose_graph_node: bad index"); return KT_ERR_INVALID; }
+    *out = c->pgo_nodes[idx];
+    return KT_OK;
 }
 
 int kt_get_deformed_slice(kt_ctx* c, int idx, kt_point_xyzrgbnormal* points, size_t max_points, size_t* count)
