@@ -434,9 +434,7 @@ int icp_frame(const IcpLevelArgs* levels, const int* iters, const float* pose12_
     const size_t stage_bytes = (size_t)6 * stage_k * FRAME_THREADS * sizeof(float);
     const bool can_stage = stage_k > 0;
     p.stage_k = stage_k;
-    static int batch_knob = -1;                     // KT_ICP_BATCH = 4 | 5 (A/B); default: 5 when the largest level leaves a remainder pass after groups of 4
-    if (batch_knob < 0) { const char* e = getenv("KT_ICP_BATCH"); batch_knob = e ? atoi(e) : 0; }
-    const int batch = batch_knob == 4 || batch_knob == 5 ? batch_knob : ((need_k % 4 == 1) ? 5 : 4);
+    const int batch = (need_k % 4 == 1) ? 5 : 4;    // 5 when the largest level leaves a remainder pass after groups of 4
     void* args[] = {&p};
     const void* fn = batch == 5 ? (const void*)icp_frame_kernel<5> : (const void*)icp_frame_kernel<4>;
     cudaError_t e = cudaLaunchCooperativeKernel(fn, dim3(grid), dim3(FRAME_THREADS), args, can_stage ? stage_bytes : 0, s);

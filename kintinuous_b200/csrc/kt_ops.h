@@ -147,8 +147,6 @@ struct IntegrateArgs {
     unsigned long long* reset_words; int reset_count, reset_stride;   // optional: reset_count 64-bit words, reset_stride apart, that the launch zeroes (the odometry's exchange words)
 };
 int integrate(const IntegrateArgs& a, float* ztable_dev /* 2*vol floats */, cudaStream_t s);
-// per-pixel colour weight (sign = normal invalid) + float RGB for IntegrateArgs::cw / rgbf; once per frame, after the normal map exists
-int color_prep(const float* nmap, const uint8_t* rgb, int rows, int cols, bool angle_color, float* cw, float4* rgbf, cudaStream_t s);
 struct RaycastArgs {
     Intr k; Mat33 R; float3 t; float trunc; float3 volume_size; const int16_t* tsdf; const uint8_t* color; int vol; int3 wrap;
     float* vmap[LEVELS]; float* nmap[LEVELS]; int rows, cols; uint8_t* vmap_color; int n_levels;   // n_levels>1: fused model pyramid

@@ -4,4 +4,3 @@ NG=${NG:-2}
 run() { echo "== $*"; env "$@" KT_BENCH_FRAMES=24 python -m torch.distributed.run --nnodes=1 --nproc-per-node $NG --master-addr 127.0.0.1 --master-port 29533 bench.py --gpus $NG --steps 60 --warmup 5 --shared-only 2>&1 | tail -1 | python tools/mg_diag.py; }
 run KT_DUMMY=1
 run KT_MG_SPLIT_ICP=1
-if [ "${MG_DIAG_MORE:-0}" = 1 ]; then run KT_MG_NO_PUBLISH=1; fi
