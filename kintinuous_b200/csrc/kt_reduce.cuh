@@ -63,8 +63,12 @@ __device__ __forceinline__ bool grid_reduce29(float (&sum)[NSUM], float* __restr
     return true;
 }
 
-__device__ __forceinline__ void accumulate_row(float (&sum)[NSUM], const float (&row)[7])
+// The only code that adds a row to the 29 sums (getProducts, reduce.cu:279-313).  S: NSUM, or the 32 of the whole-frame kernels,
+// which transpose-reduce a full warp's worth of components.
+template <int S>
+__device__ __forceinline__ void accumulate_row(float (&sum)[S], const float (&row)[7])
 {
+    static_assert(S >= NSUM, "accumulate_row: fewer than 29 sums");
     int k = 0;
 #pragma unroll
     for (int a = 0; a < 6; ++a)

@@ -70,7 +70,7 @@ struct DataTerm { short2 zero; short2 one; float diff; bool valid; };
 struct ResidualParams { RgbLevelArgs a; OdomState* st; int* partials; };
 
 // (K R K^-1, K t) from the inverse of the running estimate (RGBDOdometry.cpp:209-231), double then float.
-__device__ inline void build_warp_T(const double* T, double fx, double fy, double cx, double cy, float* krkinv, float* kt)
+__device__ inline void build_warp(const double* T, double fx, double fy, double cx, double cy, float* krkinv, float* kt)
 {
     double R[9], t[3];
     for (int i = 0; i < 3; ++i) for (int j = 0; j < 3; ++j) R[i * 3 + j] = T[j * 4 + i];          // R^T
@@ -83,9 +83,66 @@ __device__ inline void build_warp_T(const double* T, double fx, double fy, doubl
     for (int a = 0; a < 3; ++a) { double s = 0; for (int k = 0; k < 3; ++k) s += K[a * 3 + k] * t[k]; kt[a] = (float)s; }
 }
 
-__device__ inline void build_warp(const OdomState* st, double fx, double fy, double cx, double cy, float* krkinv, float* kt)
+// Pose-independent half of a photometric correspondence (reduce.cu:709-733): the 4x4 neighbourhood of the next image, the gradient
+// magnitude and the next depth of pixel idx.  Returns 0 for a pixel that cannot correspond, else 1 | I_next << 8, with its gradient in gr
+// and its depth in d1.
+__device__ __forceinline__ unsigned int rgb_precheck(const RgbLevelArgs& a, int idx, short2& gr, float& d1)
 {
-    build_warp_T(st->resultRt, fx, fy, cx, cy, krkinv, kt);
+    const int cols = a.cols, rows = a.rows;
+    const int i = idx / cols, j0 = idx - i * cols;
+    if (!(j0 < cols - 5 && i < rows - 1)) return 0;
+    bool valid = true;
+    for (int u = max(i - 2, 0); u < min(i + 2, rows); u++)
+        for (int v = max(j0 - 2, 0); v < min(j0 + 2, cols); v++)
+            valid = valid && (a.next_image[(size_t)u * cols + v] > 0);
+    if (!valid) return 0;
+    gr.x = a.dIdx[idx]; gr.y = a.dIdy[idx];
+    float mTwo = (gr.x * gr.x) + (gr.y * gr.y);
+    if (!(mTwo >= a.min_scale)) return 0;
+    d1 = a.next_depth[idx];
+    if (isnan(d1)) return 0;
+    return 1u | ((unsigned int)a.next_image[idx] << 8);
+}
+
+// Per-iteration half (reduce.cu:735-764): warp pixel (x, y) at next depth d1 into the last frame with (K R K^-1, K t) and test the last
+// frame's depth and intensity there.  True for a correspondence, with its last-frame pixel (u0, v0), depth d0 and diff = I_next - I_last.
+__device__ __forceinline__ bool rgb_correspond(const Mat33& krkinv, const float3& kt, int x, int y, float d1, unsigned int i_next,
+                                               const float* __restrict__ lastDepth, const uint8_t* __restrict__ lastImage, int cols, int rows,
+                                               float maxDepthDelta, int& u0, int& v0, float& d0, float& diff)
+{
+    float transformed_d1 = (float)(d1 * (krkinv.r2.x * x + krkinv.r2.y * y + krkinv.r2.z) + kt.z);
+    u0 = __float2int_rn((d1 * (krkinv.r0.x * x + krkinv.r0.y * y + krkinv.r0.z) + kt.x) / transformed_d1);
+    v0 = __float2int_rn((d1 * (krkinv.r1.x * x + krkinv.r1.y * y + krkinv.r1.z) + kt.y) / transformed_d1);
+    if (!(u0 >= 0 && v0 >= 0 && u0 < cols && v0 < rows)) return false;
+    d0 = __ldg(&lastDepth[(size_t)v0 * cols + u0]);
+    const unsigned int il = __ldg(&lastImage[(size_t)v0 * cols + u0]);
+    if (!(d0 > 0 && fabsf(transformed_d1 - d0) <= maxDepthDelta && il != 0)) return false;
+    diff = static_cast<float>(i_next) - static_cast<float>(il);
+    return true;
+}
+
+// One Jacobian row of RGBReduction (reduce.cu:443-480), added to sum: robust weight 1/(sigma + |diff|) (1 when sigma == -1), the next
+// image's gradient (gx, gy) and the last frame's point.
+template <int S>
+__device__ __forceinline__ void rgb_pixel_row(float sigma, float diff, short gx, short gy, const float3& cloudPoint, float sobelScale, float fx, float fy,
+                                              float (&sum)[S])
+{
+    float w = sigma + fabsf(diff);
+    w = w > 1.19209290E-07F ? 1.0f / w : 1.0f;
+    if (sigma == -1) w = 1;
+    float row[7];
+    row[6] = -w * diff;
+    float invz = 1.0 / cloudPoint.z;
+    float dI_dx_val = w * sobelScale * gx;
+    float dI_dy_val = w * sobelScale * gy;
+    float v0 = dI_dx_val * fx * invz;
+    float v1 = dI_dy_val * fy * invz;
+    float v2 = -(v0 * cloudPoint.x + v1 * cloudPoint.y) * invz;
+    row[0] = v0; row[1] = v1; row[2] = v2;
+    row[3] = -cloudPoint.z * v1 + cloudPoint.y * v2;
+    row[4] = cloudPoint.z * v0 - cloudPoint.x * v2;
+    row[5] = -cloudPoint.y * v0 + cloudPoint.x * v1;
+    accumulate_row(sum, row);
 }
 
 __global__ void __launch_bounds__(RED_THREADS)
@@ -96,57 +153,31 @@ residual_kernel(const ResidualParams p, int use_state_warp)
     __shared__ bool s_last;
     const int tid = threadIdx.x;
     if (tid == 0) {
-        if (use_state_warp) build_warp(p.st, p.a.Kfx, p.a.Kfy, p.a.Kcx, p.a.Kcy, s_w, s_w + 9);
+        if (use_state_warp) build_warp(p.st->resultRt, p.a.Kfx, p.a.Kfy, p.a.Kcx, p.a.Kcy, s_w, s_w + 9);
         else { for (int k = 0; k < 9; ++k) s_w[k] = p.st->krkinv[k]; for (int k = 0; k < 3; ++k) s_w[9 + k] = p.st->kt[k]; }
     }
     __syncthreads();
-    const float k00 = s_w[0], k01 = s_w[1], k02 = s_w[2], k10 = s_w[3], k11 = s_w[4], k12 = s_w[5], k20 = s_w[6], k21 = s_w[7], k22 = s_w[8];
+    const Mat33 krkinv = mat33_rows(s_w);
     const float3 kt = make_float3(s_w[9], s_w[10], s_w[11]);
     const int cols = p.a.cols, rows = p.a.rows, N = cols * rows;
-    const int16_t* __restrict__ dIdx = p.a.dIdx; const int16_t* __restrict__ dIdy = p.a.dIdy;
-    const float* __restrict__ lastDepth = p.a.last_depth; const float* __restrict__ nextDepth = p.a.next_depth;
-    const uint8_t* __restrict__ lastImage = p.a.last_image; const uint8_t* __restrict__ nextImage = p.a.next_image;
     DataTerm* __restrict__ corresImg = (DataTerm*)p.a.corres;
-    const float minScale = p.a.min_scale, maxDepthDelta = p.a.max_depth_delta;
 
     int2 sum = {0, 0};
     for (int k = blockIdx.x * RED_THREADS + tid; k < N; k += gridDim.x * RED_THREADS) {
-        int i = k / cols;
-        int j0 = k - (i * cols);
+        const int y = k / cols, x = k - y * cols;
         int2 value = {0, 0};
         DataTerm corres;
         corres.zero = make_short2(0, 0); corres.one = make_short2(0, 0); corres.diff = 0.f;
         corres.valid = false;
-        if (j0 < cols - 5 && i < rows - 1) {
-            bool valid = true;
-            for (int u = max(i - 2, 0); u < min(i + 2, rows); u++)
-                for (int v = max(j0 - 2, 0); v < min(j0 + 2, cols); v++)
-                    valid = valid && (nextImage[(size_t)u * cols + v] > 0);
-            if (valid) {
-                short valx = dIdx[(size_t)i * cols + j0];
-                short valy = dIdy[(size_t)i * cols + j0];
-                float mTwo = (valx * valx) + (valy * valy);
-                if (mTwo >= minScale) {
-                    int y = i, x = j0;
-                    float d1 = nextDepth[(size_t)y * cols + x];
-                    if (!isnan(d1)) {
-                        float transformed_d1 = (float)(d1 * (k20 * x + k21 * y + k22) + kt.z);
-                        int u0 = __float2int_rn((d1 * (k00 * x + k01 * y + k02) + kt.x) / transformed_d1);
-                        int v0 = __float2int_rn((d1 * (k10 * x + k11 * y + k12) + kt.y) / transformed_d1);
-                        if (u0 >= 0 && v0 >= 0 && u0 < cols && v0 < rows) {
-                            float d0 = lastDepth[(size_t)v0 * cols + u0];
-                            if (d0 > 0 && fabsf(transformed_d1 - d0) <= maxDepthDelta && lastImage[(size_t)v0 * cols + u0] != 0) {
-                                corres.zero.x = u0; corres.zero.y = v0;
-                                corres.one.x = x; corres.one.y = y;
-                                corres.diff = static_cast<float>(nextImage[(size_t)y * cols + x]) - static_cast<float>(lastImage[(size_t)v0 * cols + u0]);
-                                corres.valid = true;
-                                value.x = 1;
-                                value.y = corres.diff * corres.diff;           // Q5: truncated to int per pixel
-                            }
-                        }
-                    }
-                }
-            }
+        short2 gr; float d1; int u0, v0; float d0, diff;
+        const unsigned int meta = rgb_precheck(p.a, k, gr, d1);
+        if (meta && rgb_correspond(krkinv, kt, x, y, d1, meta >> 8, p.a.last_depth, p.a.last_image, cols, rows, p.a.max_depth_delta, u0, v0, d0, diff)) {
+            corres.zero.x = u0; corres.zero.y = v0;
+            corres.one.x = x; corres.one.y = y;
+            corres.diff = diff;
+            corres.valid = true;
+            value.x = 1;
+            value.y = diff * diff;           // Q5: truncated to int per pixel
         }
         corresImg[k] = corres;
         sum.x += value.x;
@@ -194,7 +225,6 @@ rgb_step_kernel(const RgbStepParams p)
     const DataTerm* __restrict__ corresImg = (const DataTerm*)p.a.corres;
     const float3* __restrict__ cloud = (const float3*)p.a.cloud;
     const int16_t* __restrict__ dIdx = p.a.dIdx; const int16_t* __restrict__ dIdy = p.a.dIdy;
-    const float fx = p.a.fx, fy = p.a.fy, sobelScale = p.a.sobel_scale;
 
     float sum[NSUM];
 #pragma unroll
@@ -202,23 +232,9 @@ rgb_step_kernel(const RgbStepParams p)
     for (int i = blockIdx.x * RED_THREADS + tid; i < N; i += gridDim.x * RED_THREADS) {
         const DataTerm corresp = corresImg[i];
         if (!corresp.valid) continue;
-        float w = sigma + fabsf(corresp.diff);
-        w = w > 1.19209290E-07F ? 1.0f / w : 1.0f;
-        if (sigma == -1) w = 1;
-        float row[7];
-        row[6] = -w * corresp.diff;
-        float3 cloudPoint = cloud[(size_t)corresp.zero.y * cols + corresp.zero.x];
-        float invz = 1.0 / cloudPoint.z;
-        float dI_dx_val = w * sobelScale * dIdx[(size_t)corresp.one.y * cols + corresp.one.x];
-        float dI_dy_val = w * sobelScale * dIdy[(size_t)corresp.one.y * cols + corresp.one.x];
-        float v0 = dI_dx_val * fx * invz;
-        float v1 = dI_dy_val * fy * invz;
-        float v2 = -(v0 * cloudPoint.x + v1 * cloudPoint.y) * invz;
-        row[0] = v0; row[1] = v1; row[2] = v2;
-        row[3] = -cloudPoint.z * v1 + cloudPoint.y * v2;
-        row[4] = cloudPoint.z * v0 - cloudPoint.x * v2;
-        row[5] = -cloudPoint.y * v0 + cloudPoint.x * v1;
-        accumulate_row(sum, row);
+        const float3 cloudPoint = cloud[(size_t)corresp.zero.y * cols + corresp.zero.x];
+        const size_t g = (size_t)corresp.one.y * cols + corresp.one.x;
+        rgb_pixel_row(sigma, corresp.diff, dIdx[g], dIdy[g], cloudPoint, p.a.sobel_scale, p.a.fx, p.a.fy, sum);
     }
     if (!grid_reduce29(sum, p.partials, &p.st->blocks_done, s_red, &s_last)) return;
 
@@ -284,8 +300,8 @@ rgbd_frame_kernel(const RgbdFrameParams p)
 {
     extern __shared__ __align__(128) float s_dyn[];
     // dynamic smem: [ICP stage: 6 x K x 512 floats (WITH_ICP)] [d1: K x 512 floats] [grad: K x 512 x short2] [meta: K x 512 x uint]
-    __shared__ float s_Rp[9], s_tp[3], s_Rpi[9], s_R[9], s_t[3], s_w[12];
-    __shared__ double s_Rt[16];
+    __shared__ FramePose s_pose;
+    __shared__ float s_w[12];
     __shared__ float s_red[FRAME_THREADS / 32][32];
     __shared__ double s_sumd[32];          // merged normal equations in double, written by the lanes that own the components
     __shared__ int s_cnt[FRAME_THREADS / 32][2];
@@ -298,29 +314,14 @@ rgbd_frame_kernel(const RgbdFrameParams p)
     short2* s_grad = reinterpret_cast<short2*>(s_d1 + (size_t)K * FRAME_THREADS);
     unsigned int* s_meta = reinterpret_cast<unsigned int*>(s_grad + (size_t)K * FRAME_THREADS);       // bit 0: precheck, bits 8..15: I_next
 
-    if (tid == 0) {
-        for (int k = 0; k < 9; ++k) { s_Rp[k] = p.pose12[k]; s_R[k] = p.pose12[k]; }
-        for (int k = 0; k < 3; ++k) { s_tp[k] = p.pose12[9 + k]; s_t[k] = p.pose12[9 + k]; }
-        mat3f_inverse(s_Rp, s_Rpi);
-        for (int k = 0; k < 16; ++k) s_Rt[k] = (k % 5 == 0) ? 1.0 : 0.0;
-        mbar_init(&s_mbar, 1);
-    }
-    __syncthreads();
     Mat33 Rprev_inv; float3 tprev;
-    Rprev_inv.r0 = make_float3(s_Rpi[0], s_Rpi[1], s_Rpi[2]); Rprev_inv.r1 = make_float3(s_Rpi[3], s_Rpi[4], s_Rpi[5]); Rprev_inv.r2 = make_float3(s_Rpi[6], s_Rpi[7], s_Rpi[8]);
-    tprev = make_float3(s_tp[0], s_tp[1], s_tp[2]);
+    frame_begin(s_pose, p.pose12, &s_mbar, Rprev_inv, tprev);
 
     int it = 0, ex = 0;                      // iteration / exchange counters (two exchanges per iteration)
     GridSumState gs; gs.prev[0] = 0ull; gs.prev[1] = 0ull;
-    // where lane l's component of the photometric sums lands in a trace record (A 6x6 row-major symmetric | b): rows of 7, 6, 5, ... entries
+    // where lane l's component of the photometric sums lands in a trace record; slots 42 / 43 hold sigma and count instead
     int trace_a = -1, trace_b = -1;
-    if ((threadIdx.x & 31) < 27) {
-        const int ln = threadIdx.x & 31;
-        int i = 0, base = 0;
-        while (ln >= base + (7 - i) && i < 6) { base += 7 - i; ++i; }
-        const int j = i + (ln - base);
-        if (j == 6) trace_a = 36 + i; else { trace_a = j * 6 + i; trace_b = i * 6 + j; }
-    }
+    if (lane < 27) trace_slots(lane, trace_a, trace_b);
     double icp_total = 0.0;                  // warp 0, lane l: grid total of ICP component l of this iteration
     unsigned int stage_parity = 0;
     for (int level = LEVELS - 1; level >= 0; --level) {
@@ -354,23 +355,7 @@ rgbd_frame_kernel(const RgbdFrameParams p)
             const int idx = (k * G + blockIdx.x) * FRAME_THREADS + tid;
             const int o = k * FRAME_THREADS + tid;
             unsigned int meta = 0; float d1 = 0.f; short2 gr = make_short2(0, 0);
-            if (idx < N) {
-                const int i = idx / cols, j0 = idx - i * cols;
-                if (j0 < cols - 5 && i < rows - 1) {
-                    bool valid = true;
-                    for (int u = max(i - 2, 0); u < min(i + 2, rows); u++)
-                        for (int v = max(j0 - 2, 0); v < min(j0 + 2, cols); v++)
-                            valid = valid && (a.next_image[(size_t)u * cols + v] > 0);
-                    if (valid) {
-                        gr.x = a.dIdx[idx]; gr.y = a.dIdy[idx];
-                        float mTwo = (gr.x * gr.x) + (gr.y * gr.y);
-                        if (mTwo >= a.min_scale) {
-                            d1 = a.next_depth[idx];
-                            if (!isnan(d1)) meta = 1u | ((unsigned int)a.next_image[idx] << 8);
-                        }
-                    }
-                }
-            }
+            if (idx < N) meta = rgb_precheck(a, idx, gr, d1);
             s_meta[o] = meta; s_d1[o] = d1; s_grad[o] = gr;
         }
         if (WITH_ICP) { mbar_wait(&s_mbar, stage_parity); stage_parity ^= 1u; }
@@ -378,13 +363,12 @@ rgbd_frame_kernel(const RgbdFrameParams p)
 
         for (int iter = 0; iter < p.iters[level]; ++iter, ++it) {
             // warp of this iteration from the running estimate (RGBDOdometry.cpp:209-231)
-            if (tid == 0) build_warp_T(s_Rt, a.Kfx, a.Kfy, a.Kcx, a.Kcy, s_w, s_w + 9);
+            if (tid == 0) build_warp(s_pose.Rt, a.Kfx, a.Kfy, a.Kcx, a.Kcy, s_w, s_w + 9);
             __syncthreads();
-            const float k00 = s_w[0], k01 = s_w[1], k02 = s_w[2], k10 = s_w[3], k11 = s_w[4], k12 = s_w[5], k20 = s_w[6], k21 = s_w[7], k22 = s_w[8];
+            const Mat33 krkinv = mat33_rows(s_w);
             const float3 kt = make_float3(s_w[9], s_w[10], s_w[11]);
-            Mat33 Rcurr; float3 tcurr;
-            Rcurr.r0 = make_float3(s_R[0], s_R[1], s_R[2]); Rcurr.r1 = make_float3(s_R[3], s_R[4], s_R[5]); Rcurr.r2 = make_float3(s_R[6], s_R[7], s_R[8]);
-            tcurr = make_float3(s_t[0], s_t[1], s_t[2]);
+            const Mat33 Rcurr = mat33_rows(s_pose.R);
+            const float3 tcurr = make_float3(s_pose.t[0], s_pose.t[1], s_pose.t[2]);
 
             // ---------------- pass A ----------------
             float sum[32];
@@ -402,18 +386,10 @@ rgbd_frame_kernel(const RgbdFrameParams p)
                         const unsigned int meta = s_meta[o];
                         if (meta & 1u) {
                             const int y = idx / cols, x = idx - y * cols;
-                            const float d1 = s_d1[o];
-                            float transformed_d1 = (float)(d1 * (k20 * x + k21 * y + k22) + kt.z);
-                            int u0 = __float2int_rn((d1 * (k00 * x + k01 * y + k02) + kt.x) / transformed_d1);
-                            int v0 = __float2int_rn((d1 * (k10 * x + k11 * y + k12) + kt.y) / transformed_d1);
-                            if (u0 >= 0 && v0 >= 0 && u0 < cols && v0 < rows) {
-                                float d0 = __ldg(&lastDepth[(size_t)v0 * cols + u0]);
-                                const unsigned int il = __ldg(&lastImage[(size_t)v0 * cols + u0]);
-                                if (d0 > 0 && fabsf(transformed_d1 - d0) <= maxDepthDelta && il != 0) {
-                                    const float diff = static_cast<float>((meta >> 8) & 0xffu) - static_cast<float>(il);
-                                    cval[k] = true; cu0[k] = u0; cv0[k] = v0; cdiff[k] = diff; cd0[k] = d0;
-                                    cnt += 1; sig += (int)(diff * diff);
-                                }
+                            int u0, v0; float d0, diff;
+                            if (rgb_correspond(krkinv, kt, x, y, s_d1[o], (meta >> 8) & 0xffu, lastDepth, lastImage, cols, rows, maxDepthDelta, u0, v0, d0, diff)) {
+                                cval[k] = true; cu0[k] = u0; cv0[k] = v0; cdiff[k] = diff; cd0[k] = d0;
+                                cnt += 1; sig += (int)(diff * diff);
                             }
                         }
                         if (WITH_ICP) {
@@ -421,7 +397,7 @@ rgbd_frame_kernel(const RgbdFrameParams p)
                             const int ps = K * FRAME_THREADS;
                             const float3 vc = make_float3(s_stage[o], s_stage[ps + o], s_stage[2 * ps + o]);
                             const float3 nc = make_float3(s_stage[3 * ps + o], s_stage[4 * ps + o], s_stage[5 * ps + o]);
-                            icp_pixel_staged(vc, nc, N, cols, rows, ia.vmap_g_prev, ia.nmap_g_prev, ia.k, Rcurr, tcurr, Rprev_inv, tprev, ia.dist_thres, ia.angle_thres, sum);
+                            icp_pixel(vc, nc, N, cols, rows, ia.vmap_g_prev, ia.nmap_g_prev, ia.k, Rcurr, tcurr, Rprev_inv, tprev, ia.dist_thres, ia.angle_thres, sum);
                         }
                     }
                 }
@@ -460,36 +436,10 @@ rgbd_frame_kernel(const RgbdFrameParams p)
 #pragma unroll
             for (int k = 0; k < RGBD_MAX_K; ++k) {
                 if (k < n_chunks && cval[k]) {
-                    const int o = k * FRAME_THREADS + tid;
-                    const float diff = cdiff[k];
-                    float w = sigma + fabsf(diff);
-                    w = w > 1.19209290E-07F ? 1.0f / w : 1.0f;
-                    if (sigma == -1) w = 1;
-                    float row[7];
-                    row[6] = -w * diff;
                     const float z = cd0[k];
-                    float3 cloudPoint;
-                    cloudPoint.x = (float)((cu0[k] - dcx) * z * invFx);
-                    cloudPoint.y = (float)((cv0[k] - dcy) * z * invFy);
-                    cloudPoint.z = z;
-                    float invz = 1.0 / cloudPoint.z;
-                    const short2 gr = s_grad[o];
-                    float dI_dx_val = w * sobelScale * gr.x;
-                    float dI_dy_val = w * sobelScale * gr.y;
-                    float v0 = dI_dx_val * fx * invz;
-                    float v1 = dI_dy_val * fy * invz;
-                    float v2 = -(v0 * cloudPoint.x + v1 * cloudPoint.y) * invz;
-                    row[0] = v0; row[1] = v1; row[2] = v2;
-                    row[3] = -cloudPoint.z * v1 + cloudPoint.y * v2;
-                    row[4] = cloudPoint.z * v0 - cloudPoint.x * v2;
-                    row[5] = -cloudPoint.y * v0 + cloudPoint.x * v1;
-                    int q = 0;
-#pragma unroll
-                    for (int aa = 0; aa < 6; ++aa)
-#pragma unroll
-                        for (int bb = aa; bb < 7; ++bb) sum[q++] += row[aa] * row[bb];
-                    sum[27] += row[6] * row[6];
-                    sum[28] += 1.f;
+                    const float3 cloudPoint = make_float3((float)((cu0[k] - dcx) * z * invFx), (float)((cv0[k] - dcy) * z * invFy), z);
+                    const short2 gr = s_grad[k * FRAME_THREADS + tid];
+                    rgb_pixel_row(sigma, cdiff[k], gr.x, gr.y, cloudPoint, sobelScale, fx, fy, sum);
                 }
             }
             { const float v = warp_transpose_sum(sum, lane); s_red[wid][lane] = v; }
@@ -509,23 +459,13 @@ rgbd_frame_kernel(const RgbdFrameParams p)
                 s_sumd[lane] = m;
                 __syncwarp();
                 if (lane == 0) {
-                    // unpack 27 sums -> symmetric A (row-major) and b, constant indices only (registers, no local memory)
                     double dA[36], db[6];
-                    {
-                        int shift = 0;
-#pragma unroll
-                        for (int i = 0; i < 6; ++i)
-#pragma unroll
-                            for (int j = i; j < 7; ++j) {
-                                const double value = s_sumd[shift++];
-                                if (j == 6) db[i] = value; else { dA[j * 6 + i] = value; dA[i * 6 + j] = value; }
-                            }
-                    }
-                    gauss_newton_update_fast(dA, db, s_Rt, s_Rp, s_tp, s_R, s_t);
+                    unpack_normal_equations(s_sumd, dA, db);
+                    gauss_newton_update_fast(dA, db, s_pose.Rt, s_pose.Rp, s_pose.tp, s_pose.R, s_pose.t);
                 }
                 if (p.trace && blockIdx.x == 0 && it < 64) {            // the photometric part alone, like the reference's A_rgb / b_rgb
                     float* t = p.trace + (size_t)it * TRACE_STRIDE;
-                    const float value = (float)total;              // component -> (row, column) worked out once per launch (trace_a / trace_b): CTA 0 is on every exchange's critical path
+                    const float value = (float)total;              // component -> slot worked out once per launch (trace_a / trace_b): CTA 0 is on every exchange's critical path
                     if (trace_a >= 0) t[trace_a] = value;
                     if (trace_b >= 0) t[trace_b] = value;
                     if (lane == 0) { t[42] = (float)rgb_sigma; t[43] = (float)rgb_count; }
@@ -535,22 +475,7 @@ rgbd_frame_kernel(const RgbdFrameParams p)
             __syncthreads();
         }
     }
-    if (blockIdx.x == 0 && tid < 12) {
-        if (tid < 9) p.st->Rcurr[tid] = s_R[tid]; else p.st->tcurr[tid - 9] = s_t[tid - 9];
-        if (tid == 0) p.st->iter = it;
-        if (p.host_pose) {
-            // the estimate also goes straight to mapped, pinned HOST memory (12 floats, the time-out flag, then a sequence number behind a
-            // system-scope fence): the host polls the sequence number instead of paying a D2H copy + stream synchronisation per frame
-            if (tid == 0) {
-                volatile float* hp = p.host_pose;
-                for (int k = 0; k < 9; ++k) hp[k] = s_R[k];
-                for (int k = 0; k < 3; ++k) hp[9 + k] = s_t[k];
-                ((volatile int*)p.host_pose)[12] = p.timeout ? *(volatile int*)p.timeout : 0;
-                __threadfence_system();
-                ((volatile unsigned int*)p.host_pose)[13] = p.host_seq;
-            }
-        }
-    }
+    frame_end(s_pose, it, p.st, p.host_pose, p.host_seq, p.timeout);
 }
 
 } // namespace
@@ -607,14 +532,12 @@ int rgbd_frame(const IcpLevelArgs* icp_levels, const RgbLevelArgs* rgb_levels, c
 {
     RgbdFrameParams p;
     p.host_pose = host_pose; p.host_seq = host_seq;
-    int total = 0;
-    for (int l = 0; l < LEVELS; ++l) { p.icp[l] = icp_levels[l]; p.rgb[l] = rgb_levels[l]; p.iters[l] = iters[l]; total += iters[l]; }
+    for (int l = 0; l < LEVELS; ++l) { p.icp[l] = icp_levels[l]; p.rgb[l] = rgb_levels[l]; p.iters[l] = iters[l]; }
     for (int k = 0; k < 12; ++k) p.pose12[k] = pose12_host[k];
     p.st = state; p.xwords = xwords_dev; p.trace = trace; p.timeout = timeout_dev; p.with_icp = with_icp;
     DeviceInfo& di = device_info();
-    const int sms = di.sm_count, smem_optin = di.smem_optin;
-    int grid = sms > 0 ? sms : 132;
-    if (grid > 255) grid = 255;                  // the exchange words count arrivals in 8 bits
+    const int smem_optin = di.smem_optin;
+    const int grid = frame_grid();
     int need_k = 0;
     for (int l = 0; l < LEVELS; ++l)
         if (iters[l] > 0) { int k = div_up(rgb_levels[l].rows * rgb_levels[l].cols, grid * FRAME_THREADS); if (k > need_k) need_k = k; }
@@ -632,7 +555,6 @@ int rgbd_frame(const IcpLevelArgs* icp_levels, const RgbLevelArgs* rgb_levels, c
                              : cudaLaunchCooperativeKernel((const void*)rgbd_frame_kernel<false>, dim3(grid), dim3(FRAME_THREADS), args, bytes, s);
     ++g_launches;
     if (e != cudaSuccess) return cuda_check(e, "cudaLaunchCooperativeKernel(rgbd_frame_kernel)", __FILE__, __LINE__);
-    (void)total;
     return 0;
 }
 

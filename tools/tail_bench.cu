@@ -59,6 +59,19 @@ __device__ __forceinline__ void do_solve_fast(const float* s_sum, double* s_Rt, 
     gauss_newton_update_fast(dA, db, s_Rt, s_Rp, s_tp, s_R, s_t);
 }
 
+// counter barrier: every CTA adds 1 and spins until all G have arrived at `target` (a multiple of G)
+__device__ __forceinline__ void grid_barrier(unsigned int* bar, unsigned int target)
+{
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        __threadfence();
+        atomicAdd(bar, 1u);
+        while ((int)(*((volatile unsigned int*)bar) - target) < 0) { }
+        __threadfence();
+    }
+    __syncthreads();
+}
+
 // ---- V0: what icp_frame_kernel does today -------------------------------------------------------------------------------
 __global__ void __launch_bounds__(T, 1) v0_kernel(P p)
 {
