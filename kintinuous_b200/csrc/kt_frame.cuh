@@ -19,7 +19,18 @@ enum { FRAME_THREADS = 512, STAGE_MAX_K = 18 };   // 18 passes x 6 planes x 2 KB
 // matters to the solve (DESIGN.md section 3.2).  Latency: one atomic to L2 plus one poll round trip after the LAST CTA arrived
 // (measured with tools/tail_bench.cu against the counter barrier + partial re-read it replaces).
 // Requirements: gridDim.x <= 255 (frame_grid); the words are zero when the launch starts (the host keeps them so, kt_tracker.cu).
-enum { XW_STRIDE = 160, XW_WORDS = 2 * 32 * XW_STRIDE };     // 1280 B apart (tools/tail_bench.cu times other strides)
+// Range: a signed 64-bit word holds round(x * 2^32), so the exchange is exact only while every per-CTA partial and every grid total stays
+// below 2^31 in magnitude; past that __double2ll_rn saturates, the word wraps, and the count byte still completes, so nothing would flag
+// it.  The ICP sums (icp_frame_kernel, exchange 1 of rgbd_frame_kernel) stay below that by geometry: every row entry is bounded by the
+// camera-to-surface distance, at most the volume's diagonal, so the largest sum is about N * 3 * volume_size^2 -- 1.3e8 for a 6 m volume
+// at 1280x960, 16x below the limit (a volume above ~25 m could reach it).  The photometric sums have no such bound (with sigma = 1, as
+// on a repeated frame, a 640x480 level-0 entry reaches ~8e12): exchange 2 of rgbd_frame_kernel carries them through grid_sum_words_wide.
+// Word sets: an exchange with counter ex uses set (ex & 1) -- the words of grid_sum_fixed, or the high words of grid_sum_words_wide --
+// and a wide exchange also set 2 + (ex & 1) for its low words.  icp_frame_kernel exchanges once per iteration (sets 0 and 1).
+// rgbd_frame_kernel exchanges twice per iteration from ex = 0, so exchange 1 (one word) always lands on set 0 and the wide exchange 2 on
+// sets 1 and 3; set 2 stays unused there.  It is kept so that grid_sum_words_wide, like grid_sum_fixed, is correct on consecutive
+// exchanges (tools/tail_bench.cu runs it so), not only when another exchange separates two wide ones.
+enum { XW_STRIDE = 160, XW_SETS = 4, XW_WORDS = XW_SETS * 32 * XW_STRIDE };     // 1280 B apart (tools/tail_bench.cu times other strides)
 
 __device__ __forceinline__ void red_add_u64(unsigned long long* p, unsigned long long v)
 { asm volatile("red.relaxed.gpu.global.add.u64 [%0], %1;" :: "l"(p), "l"(v) : "memory"); }
@@ -64,6 +75,38 @@ __device__ __forceinline__ double from_fixed32(long long t) { return (double)t *
 __device__ __forceinline__ double grid_sum_words(unsigned long long* words, int ex, int lane, float partial, GridSumState& st, unsigned int G, int* timeout)
 {
     return from_fixed32(grid_sum_fixed(words, ex, lane, lane < NSUM, to_fixed32(partial), st, G, timeout));
+}
+
+// grid_sum_words over two self-counting words per component, for partials beyond the 2^31 range of one: hi = rint(partial) in units of 1
+// (shifted past the count byte) and lo = to_fixed32(partial - hi), where partial - hi is exact in float.  hi * 2^32 + lo equals
+// to_fixed32(partial) exactly whenever that is in range, and the total hi_tot + lo_tot * 2^-32 is ONE correctly rounded double addition of
+// the same exact integer sum scaled by 2^-32, so every result grid_sum_words could represent comes back bit-identical; the range grows to
+// 2^55.  st_lo keeps the low words' state as st keeps the high words'.  Both words are added, then polled together: one round trip.
+__device__ __forceinline__ double grid_sum_words_wide(unsigned long long* words, int ex, int lane, float partial, GridSumState& st, GridSumState& st_lo,
+                                                      unsigned int G, int* timeout)
+{
+    if (lane >= NSUM) return 0.0;
+    const int par = ex & 1;
+    unsigned long long* wh = words + ((size_t)par * 32 + lane) * XW_STRIDE;
+    unsigned long long* wl = words + ((size_t)(2 + par) * 32 + lane) * XW_STRIDE;
+    const float hi = rintf(partial);
+    red_add_u64(wh, (unsigned long long)(__float2ll_rn(hi) * 256 + 1));
+    red_add_u64(wl, (unsigned long long)(to_fixed32(partial - hi) + 1));
+    const unsigned long long prev_h = par ? st.prev[1] : st.prev[0], prev_l = par ? st_lo.prev[1] : st_lo.prev[0];
+    unsigned long long now_h, now_l, dh, dl;
+    unsigned int spins = 0; long long t0 = 0;
+    for (;;) {
+        now_h = ld_relaxed_u64(wh); now_l = ld_relaxed_u64(wl);
+        dh = now_h - prev_h; dl = now_l - prev_l;
+        if ((unsigned int)(dh & 0xFFull) == G && (unsigned int)(dl & 0xFFull) == G) break;
+        if ((++spins & 0x3FFFu) == 0) {
+            const long long t = clock64();
+            if (t0 == 0) t0 = t;
+            else if (t - t0 > 4000000000LL) { if (timeout) *timeout = 1; break; }
+        }
+    }
+    if (par) { st.prev[1] = now_h; st_lo.prev[1] = now_l; } else { st.prev[0] = now_h; st_lo.prev[0] = now_l; }
+    return (double)((long long)(dh - (unsigned long long)G) >> 8) + from_fixed32((long long)(dl - (unsigned long long)G));
 }
 
 

@@ -357,11 +357,11 @@ int icp_frame(const IcpLevelArgs* levels, const int* iters, const float* pose12_
 namespace { __global__ void __launch_bounds__(64) zero_words_kernel(unsigned long long* w, int n, int stride) { for (int i = threadIdx.x; i < n; i += blockDim.x) w[(size_t)i * stride] = 0ull; } }
 
 size_t odom_exchange_words() { return (size_t)XW_WORDS; }
-int odom_exchange_used(int* stride) { if (stride) *stride = XW_STRIDE; return 64; }
+int odom_exchange_used(int* stride) { if (stride) *stride = XW_STRIDE; return XW_SETS * 32; }
 
 int odom_exchange_reset(unsigned long long* xwords_dev, cudaStream_t s)
 {
-    zero_words_kernel<<<1, 64, 0, s>>>(xwords_dev, 64, XW_STRIDE);
+    zero_words_kernel<<<1, 64, 0, s>>>(xwords_dev, XW_SETS * 32, XW_STRIDE);
     KT_LAUNCH_CHECK();
     return 0;
 }

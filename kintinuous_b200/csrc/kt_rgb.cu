@@ -284,7 +284,7 @@ struct RgbdFrameParams {
     int iters[LEVELS];
     float pose12[12];
     OdomState* st;
-    unsigned long long* xwords;    // grid_sum_fixed exchange words (kt_frame.cuh), zero at launch
+    unsigned long long* xwords;    // exchange words (kt_frame.cuh, XW_WORDS), zero at launch
     float* trace;
     int* timeout;
     float* host_pose; unsigned int host_seq;      // optional mapped host record: pose (12), time-out (1), sequence number (1)
@@ -319,6 +319,7 @@ rgbd_frame_kernel(const RgbdFrameParams p)
 
     int it = 0, ex = 0;                      // iteration / exchange counters (two exchanges per iteration)
     GridSumState gs; gs.prev[0] = 0ull; gs.prev[1] = 0ull;
+    GridSumState gs_lo = gs;                 // low words of exchange 2 (grid_sum_words_wide)
     // where lane l's component of the photometric sums lands in a trace record; slots 42 / 43 hold sigma and count instead
     int trace_a = -1, trace_b = -1;
     if (lane < 27) trace_slots(lane, trace_a, trace_b);
@@ -448,7 +449,8 @@ rgbd_frame_kernel(const RgbdFrameParams p)
                 float v = 0.f;
 #pragma unroll
                 for (int w = 0; w < FRAME_THREADS / 32; ++w) v += s_red[w][lane];
-                const double total = grid_sum_words(p.xwords, ex, lane, v, gs, (unsigned int)G, p.timeout);      // exchange 2: the photometric sums
+                // exchange 2: the photometric sums, two words per component (their range is not bounded by geometry, kt_frame.cuh)
+                const double total = grid_sum_words_wide(p.xwords, ex, lane, v, gs, gs_lo, (unsigned int)G, p.timeout);
                 // A = A_rgb + 100 A_icp, b = b_rgb + 10 b_icp in double (RGBDOdometry.cpp:316-321); the b sums are components
                 // 6, 12, 17, 21, 24, 26 of the 27 (internal.h:101-106 order)
                 double m = total;

@@ -694,6 +694,15 @@ int kt_create(const kt_config* cfg, kt_ctx** out)
         const int icp[4] = {10, 5, 4, 0}, icpf[4] = {0, 10, 5, 0}, rgb[4] = {10, 7, 7, 7}, rgbf[4] = {0, 10, 7, 0}, ri[4] = {10, 5, 4, 0}, rif[4] = {0, 10, 7, 0};
         const int* sel = cfg->odometry == 0 ? (cfg->fast_odometry ? icpf : icp) : cfg->odometry == 1 ? (cfg->fast_odometry ? rgbf : rgb) : (cfg->fast_odometry ? rif : ri);
         for (int i = 0; i < 4; ++i) c->iterations[i] = sel[i];
+        // KT_ODOM_ITERATIONS=i0,i1,i2,i3 (test hook, finest level first): another schedule.  With one iteration on one level and none
+        // elsewhere, the tracked frame's normal equations are those of that level at the previous pose, which a reference can rebuild.
+        // Read at every create, so that one process can make trackers with different schedules.
+        if (const char* e = getenv("KT_ODOM_ITERATIONS")) {
+            int v[4];
+            if (sscanf(e, "%d,%d,%d,%d", &v[0], &v[1], &v[2], &v[3]) != 4 || v[0] < 0 || v[1] < 0 || v[2] < 0 || v[3] < 0) {
+                delete c; set_error("kt_create: KT_ODOM_ITERATIONS must be four non-negative integers i0,i1,i2,i3"); return KT_ERR_INVALID; }
+            for (int i = 0; i < 4; ++i) c->iterations[i] = v[i];
+        }
     }
     int r = 0;
 #define KT_TRY(x) do { r = (x); if (r) { kt_destroy(c); return r; } } while (0)

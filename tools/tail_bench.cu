@@ -358,6 +358,35 @@ __global__ void __launch_bounds__(T, 1) v6_kernel(P p)
     if (tid == 0 && blockIdx.x == 0) p.out[0] = chk;
 }
 
+// ---- V7: the exchanges the odometry kernels use (kt_frame.cuh, words XW_STRIDE apart): grid_sum_words, one word per component, against
+// grid_sum_words_wide, two (the photometric sums of rgbd_frame_kernel, whose range one word cannot hold). -------------------------------
+template <int WIDE>
+__global__ void __launch_bounds__(T, 1) v7_kernel(P p)
+{
+    __shared__ float s_sum[32]; __shared__ double s_Rt[16]; __shared__ float s_Rp[9], s_tp[3], s_R[9], s_t[3];
+    const int tid = threadIdx.x, G = gridDim.x;
+    if (tid == 0) { for (int k = 0; k < 16; ++k) s_Rt[k] = (k % 5 == 0); for (int k = 0; k < 9; ++k) { s_Rp[k] = (k % 4 == 0); s_R[k] = s_Rp[k]; } for (int k = 0; k < 3; ++k) { s_tp[k] = 3.f; s_t[k] = 3.f; } }
+    __syncthreads();
+    float chk = 0.f;
+    GridSumState st; st.prev[0] = 0ull; st.prev[1] = 0ull;
+    GridSumState st_lo = st;
+    for (int it = 0; it < p.iters; ++it) {
+        long long t0 = clock64();
+        if (tid < 32) {
+            const float v = tid < NS ? my_value(tid, it) + s_t[0] * 1e-9f : 0.f;
+            const double tot = WIDE ? grid_sum_words_wide(p.ll, it, tid, v, st, st_lo, (unsigned int)G, nullptr)
+                                    : grid_sum_words(p.ll, it, tid, v, st, (unsigned int)G, nullptr);
+            if (tid < NS) s_sum[tid] = (float)tot;
+        }
+        __syncthreads();
+        if (tid == 0 && p.solve) do_solve(s_sum, s_Rt, s_Rp, s_tp, s_R, s_t);
+        __syncthreads();
+        chk += s_sum[5] + s_t[1];
+        if (blockIdx.x == 0 && tid == 0) p.cycles[it] = clock64() - t0;
+    }
+    if (tid == 0 && blockIdx.x == 0) p.out[0] = chk;
+}
+
 // ---- the solve alone, on one thread of one CTA, sums in shared memory ---------------------------------------------------
 template <int FAST> __global__ void solve_only_kernel(P p)
 {
@@ -442,6 +471,8 @@ int main()
         run("V6 stride 256 B, 16 CTAs", v6_kernel<32, 0>, p, 16, 1, true);
         run("V6 stride 256 B, 32 CTAs", v6_kernel<32, 0>, p, 32, 1, true);
         run("V6 stride 256 B, 74 CTAs", v6_kernel<32, 0>, p, 74, 1, true);
+        run("V7 grid_sum_words (one word)", v7_kernel<0>, p, sms, 1, true);
+        run("V7 grid_sum_words_wide (two words)", v7_kernel<1>, p, sms, 1, true);
         run("V4 two-level LL, 4 reducers", v4_kernel<4>, p, sms, 1, true);
         run("V4 two-level LL, 8 reducers", v4_kernel<8>, p, sms, 1, true);
         run("V4 two-level LL, 12 reducers", v4_kernel<12>, p, sms, 1, true);
