@@ -237,6 +237,61 @@ typedef struct kt_loop_report {
 KT_API int kt_close_loop(kt_ctx* ctx, const kt_loop_constraint* loop, float pose_spacing, float node_spacing, double isam_thresh,
                          kt_loop_report* report);
 KT_API int kt_num_loops(kt_ctx* ctx);                                      /* accepted loops since the last reset */
+/* Loop DETECTION: the reference's place-recognition thread (backend/PlaceRecognition.cpp) as two calls.
+ *   - kt_set_loop_detection(ctx, p) with p->enabled = 1: from the next frame on, keyframes are captured -- the first frame, every frame
+ *     whose (|rodrigues(Rcurr^-1 R_last)| + |g_curr - g_last|) / 2 >= 0.15 since the last keyframe, and every frame that shifts the volume
+ *     (KintinuousTracker.cpp:605-624, 706-718).  A keyframe's raw depth is copied and its SURF keypoints / descriptors (hessian 400,
+ *     4 octaves, 2 layers, 64-d) computed on a side stream, with no host synchronisation on the frame path; its dense pose gets
+ *     is_loop_pose = 1.  A full store (max_keyframes) stops adding; kt_num_keyframes reports it.  Disabled (the default): nothing is
+ *     allocated or launched.  NULL or enabled = 0 disables and frees the store.  Enabling allocates the store on the device up front:
+ *     max_keyframes x (rows x cols x 2 B of depth + max_features x 292 B of keypoints, descriptors and 3-D points) plus a few frames of
+ *     scratch -- about 0.9 GB at 640 x 480 with the defaults.
+ *   - kt_detect_loops processes every keyframe captured since the last call, in order (PlaceRecognition::process): exhaustive
+ *     ratio-test retrieval (0.49 on squared distances) against every keyframe at least exclude_recent older -> the one with the most
+ *     passes (>= 40, ties to the older); 3-D matches of that pair (>= 40); PnP RANSAC (500 hypotheses, 2 px) with inlier ratio >
+ *     inlier_ratio; the product's projective point-to-plane ICP between the two keyframes' depth maps, bootstrapped by PnP; fitness (mean
+ *     squared nearest-neighbour distance of the old keyframe's 2.5-voxel-filtered cloud, aligned, to the new one's) < 0.01 m^2.  With
+ *     close = 1 each loop found goes to kt_close_loop (pose_spacing, node_spacing, isam_thresh), and a loop it ACCEPTS starts the
+ *     loop_throttle_s throttle (frame timestamps; keyframes within it are not tried), as the reference's backend does; a rejected loop
+ *     starts none.  With close = 0 the library cannot know the outcome: every loop found starts the throttle.  One kt_place_result per keyframe, at most `capacity` (the rest stay pending); the
+ *     inlier pointers of a result's constraint stay valid until the next call.  world > 1: KT_ERR_INVALID. */
+typedef struct kt_loop_detection_params {
+    int enabled;
+    float inlier_ratio;          /* -il, 0.35 */
+    double loop_throttle_s;      /* -lt, 30 (frame timestamps) */
+    double isam_thresh;          /* -it, 10 */
+    float node_spacing;          /* -dg, 0.8 */
+    float pose_spacing;          /* -fl: 0 = every pose */
+    int max_keyframes;           /* 1000 */
+    int max_features;            /* 1000 per keyframe */
+    int exclude_recent;          /* 20 */
+    int close;                   /* 1: kt_close_loop every loop found */
+} kt_loop_detection_params;
+typedef enum kt_place_stage {
+    KT_PLACE_LOOP = 0,           /* a loop constraint was produced */
+    KT_PLACE_THROTTLED = 1,      /* within loop_throttle_s of the last loop */
+    KT_PLACE_NO_CANDIDATE = 2,   /* no keyframe old enough with >= 40 ratio-test passes */
+    KT_PLACE_MATCHES = 3,        /* fewer than 40 3-D matches */
+    KT_PLACE_INLIERS = 4,        /* PnP inlier ratio <= inlier_ratio */
+    KT_PLACE_FITNESS = 5         /* ICP fitness >= 0.01 */
+} kt_place_stage;
+typedef struct kt_place_result {
+    int keyframe; uint64_t time;         /* the keyframe processed */
+    int candidate; uint64_t candidate_time;   /* -1 / 0: none */
+    int passes, matches, inliers;
+    float inlier_ratio;
+    double fitness;                      /* -1 when not reached */
+    int stage;                           /* kt_place_stage */
+    kt_loop_constraint constraint;       /* stage KT_PLACE_LOOP: time1 = time, time2 = candidate_time */
+    int closed;                          /* close = 1 and kt_close_loop accepted it */
+    kt_loop_report report;               /* kt_close_loop's report (close = 1) */
+} kt_place_result;
+KT_API int kt_default_loop_detection(kt_loop_detection_params* p);
+KT_API int kt_set_loop_detection(kt_ctx* ctx, const kt_loop_detection_params* p);
+KT_API int kt_detect_loops(kt_ctx* ctx, kt_place_result* out, size_t capacity, size_t* n_out);
+/* Keyframes captured since the last reset (full = 1 once the store refused one); kt_get_keyframe waits for that keyframe's capture. */
+KT_API int kt_num_keyframes(kt_ctx* ctx, int* full);
+KT_API int kt_get_keyframe(kt_ctx* ctx, int idx, uint64_t* timestamp, int* dense_pose_index, int* n_features);
 /* The optimised nodes of the last accepted loop (timestamp, world-frame pose, is_loop_pose = named by a loop): the corrected
  * trajectory (iSAMInterface::getCameraPoses, :169-182).  0 nodes before any accepted loop. */
 KT_API int kt_num_pose_graph_nodes(kt_ctx* ctx);
@@ -400,6 +455,28 @@ typedef struct kt_pgo_report {
 } kt_pgo_report;
 KT_API int kt_op_pgo_optimise(const double* poses_dev, int n_nodes, const kt_pgo_factor* factors_dev, int n_factors, double* out_dev,
                               kt_pgo_report* report, void* stream);
+/* ---- place-recognition operators (what kt_detect_loops runs; device pointers) ----
+ * kt_op_surf -- cv::SURF(400, 4, 2, false) on the grey image (PlaceRecognition.cpp:51-88, DBowInterfaceSurf.cpp:72-99), restated from
+ * Bay et al. 2008 (kt_surf.cu header): rgb rows*cols*3 -> at most max_features keypoints, strongest first (ties by octave, layer,
+ * position), kp 6 floats each (x, y, size, angle in radians, response, laplacian sign), desc 64 floats each; *n_out (host). */
+KT_API int kt_op_surf(const uint8_t* rgb_dev, int rows, int cols, float hessian_threshold, int max_features, float* kp_dev, float* desc_dev,
+                      int* n_out, void* stream);
+/* kt_op_match_ratio -- the ratio test of Surf3DTools::surfMatch3D (Surf3DTools.h:105-140) with an exact 2-NN in place of FLANN, and the
+ * retrieval kt_detect_loops runs with it: the database is n_seg segments (keyframes) of `stride` rows of 64 floats, of which the first
+ * seg_counts[g] are valid (host array; NULL: all).  For each valid row the two nearest of n_query query descriptors (squared distances),
+ * best index and pass = d1 < ratio d2 (an invalid row: best -1, pass 0); seg_passes (host, n_seg ints, may be NULL): passes per segment. */
+KT_API int kt_op_match_ratio(const float* db_dev, int n_seg, int stride, const int* seg_counts, const float* query_dev, int n_query, float ratio,
+                             int* best_dev, float* d1_dev, float* d2_dev, uint8_t* pass_dev, int* seg_passes, void* stream);
+/* kt_op_pnp_ransac -- PNPSolver::getRelativePose / cv::solvePnPRansac (PNPSolver.cpp:51-75): n matches of new-camera xyz (p_new) with
+ * old-camera xyz (p_old) and old-image pixels (uv_old), host arrays.  pose12 (host): R row-major and t of p_old ~ R p_new + t; inliers
+ * (host, n bytes); *n_inliers. */
+KT_API int kt_op_pnp_ransac(const float* p_new, const float* p_old, const float* uv_old, int n, const float* intr4, int iterations,
+                            float threshold_px, uint64_t seed, double* pose12, uint8_t* inliers, int* n_inliers);
+/* kt_op_cloud_fitness -- IterativeClosestPoint::getFitnessScore after PlaceRecognition::icpDepthFrames (PlaceRecognition.cpp:238-276):
+ * both depth images (device, u16 mm) as clouds, voxel-grid filtered at leaf, source moved by T12 (3 x 4 row-major, host), mean squared
+ * distance to the nearest target point. */
+KT_API int kt_op_cloud_fitness(const uint16_t* src_depth_dev, const uint16_t* dst_depth_dev, int rows, int cols, const float* intr4, float leaf,
+                               const float* T12, double* fitness, size_t* n_src, size_t* n_dst);
 /* clearVolume{X,Y,Z}[Back] + ...c on both volumes (tsdf_volume.cu:117-448). axis 0..2, back 0/1. */
 KT_API int kt_op_clear_volume(int axis, int back, int16_t* tsdf_dev, uint8_t* color_dev, int vol, int current_wrap, int delta_wrap, void* stream);
 /* initVolume + initColorVolume (tsdf_volume.cu:469, :77) */

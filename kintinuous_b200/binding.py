@@ -103,6 +103,35 @@ class LoopReport(C.Structure):
         return d
 
 
+class LoopDetectionParams(C.Structure):
+    """kt_loop_detection_params (kt_default_loop_detection gives the reference's defaults)."""
+    _fields_ = [("enabled", C.c_int), ("inlier_ratio", C.c_float), ("loop_throttle_s", C.c_double), ("isam_thresh", C.c_double),
+                ("node_spacing", C.c_float), ("pose_spacing", C.c_float), ("max_keyframes", C.c_int), ("max_features", C.c_int),
+                ("exclude_recent", C.c_int), ("close", C.c_int)]
+
+
+class PlaceResult(C.Structure):
+    """kt_place_result of kt_detect_loops: one per keyframe processed."""
+    _fields_ = [("keyframe", C.c_int), ("time", C.c_uint64), ("candidate", C.c_int), ("candidate_time", C.c_uint64), ("passes", C.c_int),
+                ("matches", C.c_int), ("inliers", C.c_int), ("inlier_ratio", C.c_float), ("fitness", C.c_double), ("stage", C.c_int),
+                ("constraint", LoopConstraint), ("closed", C.c_int), ("report", LoopReport)]
+
+    STAGES = ("loop", "throttled", "no_candidate", "matches", "inliers", "fitness")
+
+    def as_dict(self):
+        d = {k: getattr(self, k) for k, _ in self._fields_ if k not in ("constraint", "report")}
+        d["stage_name"] = self.STAGES[self.stage]
+        d["constraint"] = np.array(self.constraint.constraint, np.float64).reshape(4, 4)
+        n = int(self.constraint.n_inliers)
+        if n:
+            d["inliers1"] = np.ctypeslib.as_array(C.cast(self.constraint.inliers1, C.POINTER(C.c_float)), shape=(n * 3,)).reshape(n, 3).copy()
+            d["inliers2"] = np.ctypeslib.as_array(C.cast(self.constraint.inliers2, C.POINTER(C.c_float)), shape=(n * 3,)).reshape(n, 3).copy()
+        else:
+            d["inliers1"] = d["inliers2"] = np.zeros((0, 3), np.float32)
+        d["report"] = self.report.as_dict()
+        return d
+
+
 class PgoReport(C.Structure):
     """kt_pgo_report of kt_op_pgo_optimise."""
     _fields_ = [("nodes", C.c_int), ("factors", C.c_int), ("loops", C.c_int), ("iterations", C.c_int),
@@ -327,6 +356,33 @@ class Tracker:
 
     def num_loops(self):
         return int(self.lib.kt_num_loops(self.h))
+
+    def set_loop_detection(self, enabled=True, **kw):
+        """kt_set_loop_detection with the reference's defaults, overridden by kw (LoopDetectionParams fields)."""
+        p = LoopDetectionParams()
+        _check(self.lib.kt_default_loop_detection(C.byref(p)))
+        p.enabled = int(enabled)
+        for k, v in kw.items():
+            setattr(p, k, v)
+        _check(self.lib.kt_set_loop_detection(self.h, C.byref(p)))
+
+    def detect_loops(self, capacity=256):
+        """kt_detect_loops: one dict per keyframe captured since the last call (PlaceResult.as_dict)."""
+        out = (PlaceResult * capacity)()
+        n = C.c_size_t(0)
+        _check(self.lib.kt_detect_loops(self.h, out, C.c_size_t(capacity), C.byref(n)))
+        return [out[i].as_dict() for i in range(n.value)]
+
+    def num_keyframes(self):
+        full = C.c_int(0)
+        n = int(self.lib.kt_num_keyframes(self.h, C.byref(full)))
+        return n, bool(full.value)
+
+    def keyframe(self, idx):
+        """(timestamp, dense-pose index, feature count) of keyframe idx."""
+        t = C.c_uint64(0); d = C.c_int(0); f = C.c_int(0)
+        _check(self.lib.kt_get_keyframe(self.h, int(idx), C.byref(t), C.byref(d), C.byref(f)))
+        return int(t.value), int(d.value), int(f.value)
 
     def pose_graph_nodes(self):
         """[(timestamp, 4x4 world-frame pose, is_loop_pose)] of the last accepted loop's optimised pose graph (empty before one)."""
@@ -581,6 +637,48 @@ class _Ops:
         _check(self._l().kt_op_pgo_optimise(_ptr(poses), n, _ptr(factors), int(factors.numel() // PGO_FACTOR_DTYPE.itemsize), _ptr(out),
                                             C.byref(rep), None))
         return rep
+
+    def surf(self, rgb, rows, cols, max_features=1000, threshold=400.0):
+        """kt_op_surf on a device RGB image: (kp float32 [n, 6] = x, y, size, angle, response, laplacian; desc float32 [n, 64])."""
+        import torch
+        kp = torch.empty(max_features * 6, dtype=torch.float32, device="cuda")
+        desc = torch.empty(max_features * 64, dtype=torch.float32, device="cuda")
+        n = C.c_int(0)
+        _check(self._l().kt_op_surf(_ptr(rgb), rows, cols, C.c_float(threshold), int(max_features), _ptr(kp), _ptr(desc), C.byref(n), None))
+        n = n.value
+        return kp[:6 * n].cpu().numpy().reshape(n, 6), desc[:64 * n].cpu().numpy().reshape(n, 64)
+
+    def match_ratio(self, db, query, ratio=0.49, stride=None, seg_counts=None):
+        """kt_op_match_ratio on device descriptors db [n_seg * stride, 64] (stride None: one segment of all rows), query [m, 64]; seg_counts:
+        valid rows per segment (None: all).  Returns host arrays (best, d1, d2, pass, passes per segment)."""
+        import torch
+        n, m = int(db.shape[0]), int(query.shape[0])
+        stride = n if stride is None else int(stride)
+        n_seg = n // stride if stride else 0
+        cnt = None if seg_counts is None else np.ascontiguousarray(np.asarray(seg_counts, np.int32))
+        sp = np.zeros(max(n_seg, 1), np.int32)
+        best = torch.empty(max(n, 1), dtype=torch.int32, device="cuda"); d1 = torch.empty(max(n, 1), dtype=torch.float32, device="cuda")
+        d2 = torch.empty(max(n, 1), dtype=torch.float32, device="cuda"); ps = torch.empty(max(n, 1), dtype=torch.uint8, device="cuda")
+        _check(self._l().kt_op_match_ratio(_ptr(db), n_seg, stride, _ptr(cnt), _ptr(query), m, C.c_float(ratio), _ptr(best), _ptr(d1), _ptr(d2),
+                                           _ptr(ps), _ptr(sp), None))
+        return best[:n].cpu().numpy(), d1[:n].cpu().numpy(), d2[:n].cpu().numpy(), ps[:n].cpu().numpy().astype(bool), sp[:n_seg]
+
+    def pnp_ransac(self, p_new, p_old, uv_old, intr, iterations=500, threshold_px=2.0, seed=0x4B696E74756F7573):
+        """kt_op_pnp_ransac on host arrays: (R 3x3, t 3, inlier mask, n_inliers) with p_old ~ R p_new + t."""
+        a, b, u = _f(p_new), _f(p_old), _f(uv_old)
+        n = len(a) // 3
+        pose = np.zeros(12, np.float64); inl = np.zeros(max(n, 1), np.uint8); ni = C.c_int(0)
+        k = _f(intr)
+        _check(self._l().kt_op_pnp_ransac(_ptr(a), _ptr(b), _ptr(u), n, _ptr(k), int(iterations), C.c_float(threshold_px), C.c_uint64(seed),
+                                          _ptr(pose), _ptr(inl), C.byref(ni)))
+        return pose[:9].reshape(3, 3), pose[9:].copy(), inl[:n].astype(bool), ni.value
+
+    def cloud_fitness(self, src_depth, dst_depth, rows, cols, intr, leaf, T):
+        """kt_op_cloud_fitness on device depth images (u16 mm): (fitness, n_src, n_dst) with source moved by T (3x4 or 4x4)."""
+        k = _f(intr); T12 = _f(np.asarray(T, np.float64)[:3, :4])
+        f = C.c_double(0); ns = C.c_size_t(0); nd = C.c_size_t(0)
+        _check(self._l().kt_op_cloud_fitness(_ptr(src_depth), _ptr(dst_depth), rows, cols, _ptr(k), C.c_float(leaf), _ptr(T12), C.byref(f), C.byref(ns), C.byref(nd)))
+        return f.value, ns.value, nd.value
 
     def clear_volume(self, axis, back, tsdf, color, vol, current, delta):
         _check(self._l().kt_op_clear_volume(axis, back, _ptr(tsdf), _ptr(color), vol, current, delta, None))

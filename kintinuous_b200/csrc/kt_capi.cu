@@ -9,6 +9,7 @@
 #include <cstddef>
 #include <mutex>
 #include <vector>
+#include <algorithm>
 
 using namespace kt;
 
@@ -23,7 +24,8 @@ cudaStream_t st(void* s) { return (cudaStream_t)s; }
 // (the device current at the call), and the calls that use it are serialised by a process-wide mutex, so operator calls from several
 // host threads / on several devices are safe, just not concurrent.
 struct OpScratch { OdomState* state; float* partials; int* ipartials; float* ztable; int ztable_n; unsigned int* counter; OdomState* host_state; SliceWorkspace slice_ws;
-                   MeshWorkspace mesh_ws; };
+                   MeshWorkspace mesh_ws; SurfWorkspace surf_ws; PnpWorkspace pnp_ws; SliceWorkspace fit_ws;
+                   int* place_ints; size_t place_ints_cap; };       // kt_op_surf / kt_op_match_ratio: counts in, counts out (grown on demand)
 enum { KT_MAX_DEVICES = 64 };
 OpScratch g_ops_dev[KT_MAX_DEVICES];
 std::mutex g_ops_mu;
@@ -318,6 +320,91 @@ int kt_op_rgb_step(const void* corres, float sigma, const float* cloud, float fx
     KT_CUDA(cudaStreamSynchronize(st(s)));
     unpack_normal_equations(sums, A_host, b_host);
     return KT_OK;
+}
+
+} // extern "C"
+
+// ---- place-recognition operators (kt_surf.cu, kt_place.cu, kt_slice.cu); synchronous ----
+namespace {
+// the operators' small integer scratch, kept between calls so that a call does not allocate
+int place_ints(size_t n, int** out)
+{
+    if (g_ops.place_ints_cap < n) {
+        if (g_ops.place_ints) cudaFree(g_ops.place_ints);
+        g_ops.place_ints = 0; g_ops.place_ints_cap = 0;
+        KT_CUDA(cudaMalloc((void**)&g_ops.place_ints, n * sizeof(int)));
+        g_ops.place_ints_cap = n;
+    }
+    *out = g_ops.place_ints;
+    return 0;
+}
+struct DevBuf {          // scratch of one operator call
+    std::vector<void*> p;
+    template <class T> int get(T** out, size_t n) { void* q = 0; KT_CUDA(cudaMalloc(&q, n ? n * sizeof(T) : 1)); p.push_back(q); *out = (T*)q; return 0; }
+    ~DevBuf() { for (void* q : p) cudaFree(q); }
+};
+}
+
+extern "C" {
+
+int kt_op_surf(const uint8_t* rgb, int rows, int cols, float thr, int max_features, float* kp, float* desc, int* n_out, void* s)
+{
+    if (!rgb || !kp || !desc || !n_out) { set_error("kt_op_surf: null argument"); return KT_ERR_INVALID; }
+    KT_OPS_LOCK();
+    int* n_dev = 0; int r;
+    if ((r = place_ints(1, &n_dev))) return r;
+    if ((r = surf(rgb, rows, cols, thr, max_features, kp, desc, n_dev, &g_ops.surf_ws, st(s)))) return r;
+    KT_CUDA(cudaMemcpyAsync(n_out, n_dev, sizeof(int), cudaMemcpyDeviceToHost, st(s)));
+    KT_CUDA(cudaStreamSynchronize(st(s)));
+    return KT_OK;
+}
+
+int kt_op_match_ratio(const float* db, int n_seg, int stride, const int* seg_counts, const float* q, int n_query, float ratio, int* best, float* d1,
+                      float* d2, uint8_t* pass, int* seg_passes, void* s)
+{
+    if (!db || !q || !best || !d1 || !d2 || !pass || n_seg < 0 || stride < 0 || n_query < 0) { set_error("kt_op_match_ratio: bad argument"); return KT_ERR_INVALID; }
+    if (n_seg == 0 || stride == 0) return KT_OK;
+    KT_OPS_LOCK();
+    int* ints = 0; int r;
+    if ((r = place_ints(2 * (size_t)n_seg + 1, &ints))) return r;
+    std::vector<int> h((size_t)n_seg + 1, stride);
+    if (seg_counts) for (int g = 0; g < n_seg; ++g) h[(size_t)g] = std::max(0, std::min(stride, seg_counts[g]));
+    h[(size_t)n_seg] = n_query;
+    KT_CUDA(cudaMemcpyAsync(ints, h.data(), h.size() * sizeof(int), cudaMemcpyHostToDevice, st(s)));
+    if ((r = match_ratio(db, n_seg, stride, ints, q, ints + n_seg, n_query, ratio, best, d1, d2, pass, seg_passes ? ints + n_seg + 1 : 0, st(s)))) return r;
+    if (seg_passes) KT_CUDA(cudaMemcpyAsync(seg_passes, ints + n_seg + 1, (size_t)n_seg * sizeof(int), cudaMemcpyDeviceToHost, st(s)));
+    KT_CUDA(cudaStreamSynchronize(st(s)));
+    return KT_OK;
+}
+
+int kt_op_pnp_ransac(const float* p_new, const float* p_old, const float* uv_old, int n, const float* k4, int iterations, float thr, uint64_t seed,
+                     double* pose12, uint8_t* inliers, int* n_inliers)
+{
+    if (!p_new || !p_old || !uv_old || !k4 || !pose12 || !inliers || !n_inliers || n < 3 || iterations < 1) { set_error("kt_op_pnp_ransac: bad argument"); return KT_ERR_INVALID; }
+    KT_OPS_LOCK();
+    DevBuf b; float *pn = 0, *po = 0, *uv = 0; double* pose = 0; unsigned char* in = 0; int* ni = 0; int r;
+    if ((r = b.get(&pn, 3 * (size_t)n)) || (r = b.get(&po, 3 * (size_t)n)) || (r = b.get(&uv, 2 * (size_t)n)) || (r = b.get(&pose, 12)) || (r = b.get(&in, (size_t)n)) || (r = b.get(&ni, 1))) return r;
+    KT_CUDA(cudaMemcpy(pn, p_new, 12 * (size_t)n, cudaMemcpyHostToDevice));
+    KT_CUDA(cudaMemcpy(po, p_old, 12 * (size_t)n, cudaMemcpyHostToDevice));
+    KT_CUDA(cudaMemcpy(uv, uv_old, 8 * (size_t)n, cudaMemcpyHostToDevice));
+    PnpArgs a; a.p_new = pn; a.p_old = po; a.uv_old = uv; a.n = n; a.k = intr4(k4); a.iterations = iterations; a.threshold_px = thr; a.seed = seed;
+    if ((r = pnp_ransac(a, &g_ops.pnp_ws, pose, in, ni, 0))) return r;
+    KT_CUDA(cudaMemcpy(pose12, pose, 12 * sizeof(double), cudaMemcpyDeviceToHost));
+    KT_CUDA(cudaMemcpy(inliers, in, (size_t)n, cudaMemcpyDeviceToHost));
+    KT_CUDA(cudaMemcpy(n_inliers, ni, sizeof(int), cudaMemcpyDeviceToHost));
+    return KT_OK;
+}
+
+int kt_op_cloud_fitness(const uint16_t* src_depth, const uint16_t* dst_depth, int rows, int cols, const float* k4, float leaf, const float* T12,
+                        double* fitness, size_t* n_src, size_t* n_dst)
+{
+    if (!src_depth || !dst_depth || !k4 || !T12 || !fitness || !n_src || !n_dst || rows <= 0 || cols <= 0) { set_error("kt_op_cloud_fitness: bad argument"); return KT_ERR_INVALID; }
+    KT_OPS_LOCK();
+    const size_t P = (size_t)rows * cols;
+    DevBuf b; kt_point_xyzrgb *cs = 0, *cd = 0; kt_point_xyzrgbnormal *os = 0, *od = 0; double* d2 = 0; int r;
+    if ((r = b.get(&cs, P)) || (r = b.get(&cd, P)) || (r = b.get(&os, P)) || (r = b.get(&od, P)) || (r = b.get(&d2, P + 8))) return r;
+    if ((r = depth_to_cloud(src_depth, rows, cols, intr4(k4), cs, 0)) || (r = depth_to_cloud(dst_depth, rows, cols, intr4(k4), cd, 0))) return r;
+    return cloud_fitness(cs, P, cd, P, leaf, T12, &g_ops.slice_ws, &g_ops.fit_ws, os, od, P, d2, fitness, n_src, n_dst, 0);
 }
 
 } // extern "C"

@@ -203,6 +203,32 @@ struct PgoFactor;
 // Gauss-Newton from poses_in (device, n x 16 FP64) into X (device, may alias) over the host factor list; every field of the report.
 // Synchronises s.
 int pgo_optimise(const double* poses_in, int n, const PgoFactor* factors, int n_factors, double* X, kt_pgo_report* rep, cudaStream_t s);
+// ---- place recognition (kt_surf.cu, kt_place.cu, cloud_fitness in kt_slice.cu; host logic in kt_place.hpp) ----
+struct SurfWorkspace {
+    int rows, cols; int* integral; float* resp; void* cand; unsigned long long* keys; unsigned int* idx; unsigned int* n_cand; void* tmp; size_t tmp_bytes;
+    SurfWorkspace() : rows(0), cols(0), integral(0), resp(0), cand(0), keys(0), idx(0), n_cand(0), tmp(0), tmp_bytes(0) {}
+};
+int surf_ws_reserve(SurfWorkspace* ws, int rows, int cols);
+void surf_ws_free(SurfWorkspace* ws);
+// RGB image -> at most max_features keypoints, strongest first: kp 6 floats each (x, y, size, angle in radians, response, laplacian sign),
+// desc 64 floats each, *n_out_dev (device) = keypoints written.  Asynchronous.
+int surf(const uint8_t* rgb, int rows, int cols, float threshold, int max_features, float* kp, float* desc, int* n_out_dev, SurfWorkspace* ws, cudaStream_t s);
+// camera-frame xyz of each keypoint (kt_place.hpp place_lookup_3d), NaN without one; max_n rows written
+int keypoints_3d(const float* kp, const int* n_dev, int max_n, const uint16_t* depth, int rows, int cols, const Intr& k, float* xyz, cudaStream_t s);
+// n_seg segments of `stride` database rows (64 floats each), segment g's first seg_count_dev[g] valid; per row the two nearest of the first
+// *n_query_dev (<= q_cap) query descriptors: best index, d1, d2 (squared), pass = d1 < ratio d2; seg_passes (may be null): passes per segment
+int match_ratio(const float* db, int n_seg, int stride, const int* seg_count_dev, const float* q, const int* n_query_dev, int q_cap, float ratio,
+                int* best, float* d1, float* d2, unsigned char* pass, int* seg_passes, cudaStream_t s);
+struct PnpArgs { const float* p_new; const float* p_old; const float* uv_old; int n; Intr k; int iterations; float threshold_px; unsigned long long seed; };
+struct PnpWorkspace { int* counts; double* hyps; unsigned int* counter; int cap; PnpWorkspace() : counts(0), hyps(0), counter(0), cap(0) {} };
+// pose12 (device, FP64): R row-major + t with R p_new + t in the old camera; inliers (device) per match; *n_inliers (device)
+int pnp_ransac(const PnpArgs& a, PnpWorkspace* ws, double* pose12, unsigned char* inliers, int* n_inliers, cudaStream_t s);
+void pnp_ws_free(PnpWorkspace* ws);
+// depth (u16 mm) -> rows*cols kt_point_xyzrgb, alpha 1 where the depth is valid
+int depth_to_cloud(const uint16_t* depth, int rows, int cols, const Intr& k, void* cloud, cudaStream_t s);
+// getFitnessScore of the loop check: d2_dev holds capacity + 8 doubles; synchronises s
+int cloud_fitness(const void* src, size_t n_src, const void* dst, size_t n_dst, float leaf, const float* T12, SliceWorkspace* ws_src, SliceWorkspace* ws_dst,
+                  void* src_out, void* dst_out, size_t capacity, double* d2_dev, double* fitness, size_t* n_src_used, size_t* n_dst_used, cudaStream_t s);
 // cross-GPU barrier: every rank writes `epoch` into slot [rank] of every peer's flag array, then waits until all slots of its own
 // array reach `epoch` (bounded spin: returns through *error_dev != 0 instead of hanging the GPU if a peer never arrives)
 int xgpu_barrier(unsigned int* const* peer_flags_dev /* [world] device array of pointers */, unsigned int* my_flags, int rank, int world,

@@ -17,6 +17,7 @@
 #include "kt_posegraph.hpp"
 #include "kt_deform.hpp"
 #include "kt_pgo.hpp"
+#include "kt_place.hpp"
 #include <cstdlib>
 #include "../../include/kintinuous_b200.h"
 #include <vector>
@@ -116,6 +117,41 @@ struct PinnedArena {
 // what the host reads back after the odometry of a frame
 struct OdomResult { float Rcurr[9]; float tcurr[3]; int timeout; unsigned int seq; int pad[2]; };     // seq: written last by the odometry kernel (mapped host memory)
 
+// Place recognition (kt_set_loop_detection / kt_detect_loops): keyframes' raw depth, SURF keypoints / descriptors and their 3-D points, captured on
+// `stream` (the frame path never waits for it on the host), and the scratch of the detection chain.  Allocated only while detection is on.
+struct PlaceStore {
+    kt_loop_detection_params p;
+    int rows, cols, maxK, maxF;
+    cudaStream_t stream; cudaEvent_t ev_input, ev_copied;
+    uint16_t* depth; uint8_t* rgb; float* kp; float* desc; float* xyz; int* nfeat_dev; int* nfeat_host;
+    SurfWorkspace surf_ws;
+    std::vector<uint64_t> times; std::vector<int> dense_idx;
+    size_t processed; bool full;
+    float lastR[9], lastG[3];
+    uint64_t last_loop;
+    // detection scratch
+    int* best; float* d1; float* d2; unsigned char* pass; int* seg_passes;
+    float* pn; float* po; float* uv; double* pose; unsigned char* inl; int* ninl; PnpWorkspace pnp_ws;
+    uint16_t* depths[2][LEVELS]; float* vmaps[2][LEVELS]; float* nmaps[2][LEVELS];
+    OdomState* state; unsigned long long* xwords; float* trace;
+    kt_point_xyzrgb* cloud[2]; kt_point_xyzrgbnormal* cent[2]; double* d2fit; SliceWorkspace ws[2];
+    std::vector<std::vector<float> > in_new, in_old;      // inliers of the results of the last kt_detect_loops
+    std::vector<void*> allocs;
+    template <class T> int alloc(T** q, size_t n) { void* v = 0; KT_CUDA(cudaMalloc(&v, n ? n * sizeof(T) : 1)); allocs.push_back(v); *q = (T*)v; return 0; }
+};
+
+static void place_free(PlaceStore* ps)
+{
+    if (!ps) return;
+    if (ps->stream) { cudaStreamSynchronize(ps->stream); cudaStreamDestroy(ps->stream); }
+    if (ps->ev_input) cudaEventDestroy(ps->ev_input);
+    if (ps->ev_copied) cudaEventDestroy(ps->ev_copied);
+    if (ps->nfeat_host) cudaFreeHost(ps->nfeat_host);
+    surf_ws_free(&ps->surf_ws); pnp_ws_free(&ps->pnp_ws); slice_ws_free(&ps->ws[0]); slice_ws_free(&ps->ws[1]);
+    for (void* q : ps->allocs) cudaFree(q);
+    delete ps;
+}
+
 } // namespace kt
 
 using namespace kt;
@@ -186,6 +222,7 @@ struct kt_ctx {
     VolumeView vv;
     float last_int_Rinv[9], last_int_t[3]; int last_int_wrap[3];       // arguments of the last integration (kt_debug_last_integrate)
     uint8_t* view_dev;                                                  // GUI taps: shaded image, colour image, model depth (allocated on first use)
+    PlaceStore* place;                                                  // loop detection (null while it is off)
 };
 
 namespace {
@@ -479,10 +516,10 @@ int build_frontend(kt_ctx* c, const uint16_t* depth_raw, const uint8_t* rgb, flo
 
 // densePoseGraph.push_back(DensePose(current_utime, [Rcurr | currentGlobalCamera], isLoopPose)); latestDensePoseId++ and, for tracked
 // frames, outputPose (KintinuousTracker.cpp:529-536, :901-914)
-void record_dense_pose(kt_ctx* c, bool first)
+void record_dense_pose(kt_ctx* c, bool first, bool keyframe)
 {
     kt_dense_pose d;
-    d.timestamp = c->current_utime; d.is_loop_pose = first ? 1 : 0;
+    d.timestamp = c->current_utime; d.is_loop_pose = (first || keyframe) ? 1 : 0;
     const M3& R = c->rmats.back();
     for (int r = 0; r < 3; ++r) { for (int k = 0; k < 3; ++k) d.pose[r * 4 + k] = R.m[r * 3 + k]; d.pose[r * 4 + 3] = c->currentGlobalCamera[r]; }
     d.pose[12] = d.pose[13] = d.pose[14] = 0.f; d.pose[15] = 1.f;
@@ -494,6 +531,36 @@ void record_dense_pose(kt_ctx* c, bool first)
     }
 }
 
+// The keyframe rule (kt_place.hpp) and, for a keyframe, its capture on the place stream: raw depth and colour copied (the compute stream
+// waits for the copy before the inputs can be reused), SURF, the keypoints' 3-D points, the feature count into pinned memory.
+int place_capture(kt_ctx* c, bool first, bool* keyframe)
+{
+    *keyframe = false;
+    PlaceStore* ps = c->place;
+    if (!ps) return 0;
+    const float* R = c->rmats.back().m;
+    const bool kf = first || ps->times.empty() || c->shifted_last > 0 || place_is_keyframe(R, ps->lastR, c->currentGlobalCamera, ps->lastG);
+    if (!kf) return 0;
+    for (int k = 0; k < 9; ++k) ps->lastR[k] = R[k];
+    for (int k = 0; k < 3; ++k) ps->lastG[k] = c->currentGlobalCamera[k];
+    if ((int)ps->times.size() >= ps->maxK) { ps->full = true; return 0; }
+    const size_t P = (size_t)ps->rows * ps->cols, k = ps->times.size();
+    const Intr K = {c->cfg.fx, c->cfg.fy, c->cfg.cx, c->cfg.cy};
+    KT_CUDA(cudaStreamWaitEvent(ps->stream, ps->ev_input, 0));
+    KT_CUDA(cudaMemcpyAsync(ps->depth + k * P, c->depth_raw, P * 2, cudaMemcpyDeviceToDevice, ps->stream));
+    KT_CUDA(cudaMemcpyAsync(ps->rgb, c->rgb, P * 3, cudaMemcpyDeviceToDevice, ps->stream));
+    KT_CUDA(cudaEventRecord(ps->ev_copied, ps->stream));
+    KT_CUDA(cudaStreamWaitEvent(c->stream, ps->ev_copied, 0));
+    float* kp = ps->kp + k * ps->maxF * 6;
+    int r;
+    if ((r = surf(ps->rgb, ps->rows, ps->cols, 400.f, ps->maxF, kp, ps->desc + k * ps->maxF * 64, ps->nfeat_dev + k, &ps->surf_ws, ps->stream))) return r;
+    if ((r = keypoints_3d(kp, ps->nfeat_dev + k, ps->maxF, ps->depth + k * P, ps->rows, ps->cols, K, ps->xyz + k * ps->maxF * 3, ps->stream))) return r;
+    KT_CUDA(cudaMemcpyAsync(ps->nfeat_host + k, ps->nfeat_dev + k, sizeof(int), cudaMemcpyDeviceToHost, ps->stream));
+    ps->times.push_back(c->current_utime); ps->dense_idx.push_back((int)c->dense_poses.size());
+    *keyframe = true;
+    return 0;
+}
+
 void mark(kt_ctx* c, int i) { if (c->timing) cudaEventRecord(c->ev[i], c->stream); }
 
 int process_frame_device(kt_ctx* c, uint64_t utime, kt_pose* out)
@@ -502,6 +569,7 @@ int process_frame_device(kt_ctx* c, uint64_t utime, kt_pose* out)
     const int mode = c->cfg.odometry;
     int r;
     c->shifted_last = 0;
+    if (c->place) KT_CUDA(cudaEventRecord(c->place->ev_input, c->stream));       // this frame's raw inputs are in place
     mark(c, 0);
     if (!c->frontend_ready) {
         // the first frame's photometric pyramids are the "last" set (RGBDOdometry::firstRun), every later frame's the "next" set
@@ -527,7 +595,9 @@ int process_frame_device(kt_ctx* c, uint64_t utime, kt_pose* out)
         mark(c, 5);
         ++c->global_time;
         c->current_utime = utime;
-        record_dense_pose(c, true);                                                      // .cpp:529-536 (no outputPose on the first frame)
+        bool kf = false;
+        if ((r = place_capture(c, true, &kf))) return r;
+        record_dense_pose(c, true, kf);                                                  // .cpp:529-536 (no outputPose on the first frame)
         if (out) kt_get_pose(c, out);
         return 0;
     }
@@ -614,7 +684,9 @@ int process_frame_device(kt_ctx* c, uint64_t utime, kt_pose* out)
     // has already fired (free to check), else with the next frame's pose read-back (run_odometry)
     if (c->world > 1 && *(volatile int*)c->mg_error_host) { set_error("cross-GPU barrier timed out waiting for rank %d", *c->mg_error_host - 1); return KT_ERR_STATE; }
     ++c->global_time;
-    record_dense_pose(c, false);                                                         // .cpp:901-914
+    bool kf = false;
+    if ((r = place_capture(c, false, &kf))) return r;                                   // .cpp:605-624, 706-718
+    record_dense_pose(c, false, kf);                                                     // .cpp:901-914
     if (out) kt_get_pose(c, out);
     return 0;
 }
@@ -646,6 +718,11 @@ int kt_reset(kt_ctx* c)
     c->deformed.clear();
     if (c->deform_arena) c->deform_arena->rewind();
     c->loops.clear(); c->pgo_nodes.clear();
+    if (c->place) {                              // reset(): the place-recognition buffer starts again (.cpp:290-298)
+        cudaStreamSynchronize(c->place->stream);
+        c->place->times.clear(); c->place->dense_idx.clear(); c->place->processed = 0; c->place->full = false; c->place->last_loop = 0;
+        c->place->in_new.clear(); c->place->in_old.clear();
+    }
     c->dense_poses.clear();                      // reset(): densePoseGraph.clear(), latestDensePoseId = 0 (.cpp:300-301)
     c->trace_iters = 0; c->shifted_last = 0; c->cloud_count = 0;
     c->pf_valid = false; c->pf_built = false; c->frontend_ready = false; c->maps_on_stream = false;
@@ -811,6 +888,7 @@ int kt_destroy(kt_ctx* c)
     if (c->stream) cudaStreamSynchronize(c->stream);
     for (int g = 0; g < MAX_GPUS; ++g) if (c->peer_arena[g] && c->peer_arena[g] != c->arena) cudaIpcCloseMemHandle(c->peer_arena[g]);
     if (c->mg_error_host) cudaFreeHost(c->mg_error_host);
+    place_free(c->place); c->place = 0;
     drop_slices(c);
     if (c->pose_log) fclose(c->pose_log);
     if (c->slice_arena) { c->slice_arena->release(); delete c->slice_arena; }
@@ -1354,6 +1432,249 @@ int kt_close_loop(kt_ctx* c, const kt_loop_constraint* loop, float pose_spacing,
 }
 
 int kt_num_loops(kt_ctx* c) { return c ? (int)c->loops.size() : 0; }
+
+// ---- loop detection (PlaceRecognition, backend/PlaceRecognition.cpp) ----
+int kt_default_loop_detection(kt_loop_detection_params* p)
+{
+    if (!p) return KT_ERR_INVALID;
+    p->enabled = 1; p->inlier_ratio = 0.35f; p->loop_throttle_s = 30.0; p->isam_thresh = 10.0; p->node_spacing = 0.8f; p->pose_spacing = 0.f;
+    p->max_keyframes = 1000; p->max_features = 1000; p->exclude_recent = 20; p->close = 1;
+    return KT_OK;
+}
+
+int kt_set_loop_detection(kt_ctx* c, const kt_loop_detection_params* p)
+{
+    if (!c) return KT_ERR_INVALID;
+    KT_CUDA(cudaSetDevice(c->cfg.device));
+    if (!p || !p->enabled) { place_free(c->place); c->place = 0; return KT_OK; }
+    if (c->world > 1) { set_error("kt_set_loop_detection: a volume shared by %d GPUs has no loop detection", c->world); return KT_ERR_INVALID; }
+    if (p->max_keyframes < 1 || p->max_features < 2 || p->exclude_recent < 1 || !(p->inlier_ratio >= 0.f) || !(p->loop_throttle_s >= 0.0)) {
+        set_error("kt_set_loop_detection: bad parameters"); return KT_ERR_INVALID;
+    }
+    if (c->place) {          // new parameters; the store is kept when its shape is unchanged
+        if (c->place->maxK == p->max_keyframes && c->place->maxF == p->max_features) { c->place->p = *p; return KT_OK; }
+        place_free(c->place); c->place = 0;
+    }
+    PlaceStore* ps = new PlaceStore();
+    ps->p = *p; ps->rows = c->cfg.rows; ps->cols = c->cfg.cols; ps->maxK = p->max_keyframes; ps->maxF = p->max_features;
+    const size_t P = (size_t)ps->rows * ps->cols, K = (size_t)ps->maxK, F = (size_t)ps->maxF;
+    int r = 0;
+#define PS_TRY(x) do { if ((r = (x))) { place_free(ps); return r; } } while (0)
+    PS_TRY(cuda_check(cudaStreamCreateWithFlags(&ps->stream, cudaStreamNonBlocking), "stream", __FILE__, __LINE__));
+    PS_TRY(cuda_check(cudaEventCreateWithFlags(&ps->ev_input, cudaEventDisableTiming), "event", __FILE__, __LINE__));
+    PS_TRY(cuda_check(cudaEventCreateWithFlags(&ps->ev_copied, cudaEventDisableTiming), "event", __FILE__, __LINE__));
+    PS_TRY(cuda_check(cudaMallocHost((void**)&ps->nfeat_host, K * sizeof(int)), "pinned", __FILE__, __LINE__));
+    PS_TRY(ps->alloc(&ps->depth, K * P)); PS_TRY(ps->alloc(&ps->rgb, P * 3)); PS_TRY(ps->alloc(&ps->kp, K * F * 6)); PS_TRY(ps->alloc(&ps->desc, K * F * 64));
+    PS_TRY(ps->alloc(&ps->xyz, K * F * 3)); PS_TRY(ps->alloc(&ps->nfeat_dev, K));
+    PS_TRY(ps->alloc(&ps->best, K * F)); PS_TRY(ps->alloc(&ps->d1, K * F)); PS_TRY(ps->alloc(&ps->d2, K * F)); PS_TRY(ps->alloc(&ps->pass, K * F));
+    PS_TRY(ps->alloc(&ps->seg_passes, K));
+    PS_TRY(ps->alloc(&ps->pn, F * 3)); PS_TRY(ps->alloc(&ps->po, F * 3)); PS_TRY(ps->alloc(&ps->uv, F * 2)); PS_TRY(ps->alloc(&ps->pose, 12));
+    PS_TRY(ps->alloc(&ps->inl, F)); PS_TRY(ps->alloc(&ps->ninl, 1));
+    for (int s2 = 0; s2 < 2; ++s2) {
+        for (int l = 0; l < LEVELS; ++l) {
+            const size_t Pl = P >> (2 * l);
+            PS_TRY(ps->alloc(&ps->depths[s2][l], Pl)); PS_TRY(ps->alloc(&ps->vmaps[s2][l], Pl * 3)); PS_TRY(ps->alloc(&ps->nmaps[s2][l], Pl * 3));
+            PS_TRY(cuda_check(cudaMemset(ps->vmaps[s2][l], 0, Pl * 12), "memset", __FILE__, __LINE__));
+            PS_TRY(cuda_check(cudaMemset(ps->nmaps[s2][l], 0, Pl * 12), "memset", __FILE__, __LINE__));
+        }
+        PS_TRY(ps->alloc(&ps->cloud[s2], P)); PS_TRY(ps->alloc(&ps->cent[s2], P));
+    }
+    PS_TRY(ps->alloc(&ps->d2fit, P + 8));
+    PS_TRY(ps->alloc(&ps->state, 1)); PS_TRY(cuda_check(cudaMemset(ps->state, 0, sizeof(OdomState)), "memset", __FILE__, __LINE__));
+    PS_TRY(ps->alloc(&ps->xwords, odom_exchange_words())); PS_TRY(ps->alloc(&ps->trace, (size_t)MAX_TRACE_ITERS * TRACE_STRIDE));
+#undef PS_TRY
+    c->place = ps;
+    return KT_OK;
+}
+
+int kt_num_keyframes(kt_ctx* c, int* full)
+{
+    if (!c) return 0;
+    if (full) *full = c->place && c->place->full ? 1 : 0;
+    return c->place ? (int)c->place->times.size() : 0;
+}
+
+int kt_get_keyframe(kt_ctx* c, int idx, uint64_t* timestamp, int* dense_pose_index, int* n_features)
+{
+    if (!c || !c->place || idx < 0 || idx >= (int)c->place->times.size()) { set_error("kt_get_keyframe: bad argument"); return KT_ERR_INVALID; }
+    KT_CUDA(cudaSetDevice(c->cfg.device));
+    KT_CUDA(cudaStreamSynchronize(c->place->stream));
+    if (timestamp) *timestamp = c->place->times[idx];
+    if (dense_pose_index) *dense_pose_index = c->place->dense_idx[idx];
+    if (n_features) *n_features = c->place->nfeat_host[idx];
+    return KT_OK;
+}
+
+namespace {
+
+// 4 x 4 row-major FP64 helpers of the detection chain
+void m4_from12(const double* p, double* T) { for (int r = 0; r < 3; ++r) { for (int k = 0; k < 3; ++k) T[r * 4 + k] = p[r * 3 + k]; T[r * 4 + 3] = p[9 + r]; } T[12] = T[13] = T[14] = 0; T[15] = 1; }
+void m4_mul(const double* A, const double* B, double* C) { for (int i = 0; i < 4; ++i) for (int j = 0; j < 4; ++j) { double s = 0; for (int k = 0; k < 4; ++k) s += A[i * 4 + k] * B[k * 4 + j]; C[i * 4 + j] = s; } }
+void m4_rigid_inverse(const double* T, double* I)
+{
+    for (int i = 0; i < 3; ++i) { for (int j = 0; j < 3; ++j) I[i * 4 + j] = T[j * 4 + i]; I[i * 4 + 3] = -(T[0 * 4 + i] * T[3] + T[1 * 4 + i] * T[7] + T[2 * 4 + i] * T[11]); }
+    I[12] = I[13] = I[14] = 0; I[15] = 1;
+}
+
+// One keyframe through the chain (PlaceRecognition::process + processLoopClosureDetection, PlaceRecognition.cpp:51-209).
+int place_process(kt_ctx* c, int q, kt_place_result* res)
+{
+    PlaceStore* ps = c->place;
+    cudaStream_t s = c->stream;
+    const size_t P = (size_t)ps->rows * ps->cols, F = (size_t)ps->maxF;
+    const float intr[4] = {c->cfg.fx, c->cfg.fy, c->cfg.cx, c->cfg.cy};
+    const Intr K = {intr[0], intr[1], intr[2], intr[3]};
+    const float RATIO = 0.49f;
+    const int MIN_PASSES = 40, MIN_MATCHES = 40, PNP_ITERS = 500;
+    std::memset(res, 0, sizeof(*res));
+    res->keyframe = q; res->time = ps->times[q]; res->candidate = -1; res->fitness = -1.0;
+    int r;
+    if (place_throttled(ps->last_loop, res->time, ps->p.loop_throttle_s)) { res->stage = KT_PLACE_THROTTLED; return 0; }
+    res->stage = KT_PLACE_NO_CANDIDATE;
+    const int nseg = q - ps->p.exclude_recent + 1;
+    if (nseg <= 0) return 0;
+    // retrieval: every feature of every keyframe old enough against the new keyframe's
+    if ((r = match_ratio(ps->desc, nseg, ps->maxF, ps->nfeat_dev, ps->desc + (size_t)q * F * 64, ps->nfeat_dev + q, ps->maxF, RATIO, ps->best, ps->d1, ps->d2,
+                         ps->pass, ps->seg_passes, s))) return r;
+    std::vector<int> passes((size_t)q + 1, 0);
+    KT_CUDA(cudaMemcpyAsync(passes.data(), ps->seg_passes, (size_t)nseg * sizeof(int), cudaMemcpyDeviceToHost, s));
+    KT_CUDA(cudaStreamSynchronize(s));
+    const int cand = place_select_candidate(passes.data(), q, ps->p.exclude_recent, MIN_PASSES);
+    if (cand < 0) return 0;
+    res->candidate = cand; res->candidate_time = ps->times[cand]; res->passes = passes[cand];
+    // 3-D matching of the pair in surfMatch3D's order (Surf3DTools.h:105-176): the ratio test over ALL features of the two stored blocks
+    // (every old feature against every new one, counts on the device), one match per new feature, then the pairs without a 3-D point
+    // dropped (kt_place.hpp place_match_3d)
+    const int nq = ps->nfeat_host[q], nc = ps->nfeat_host[cand];
+    if ((r = match_ratio(ps->desc + (size_t)cand * F * 64, 1, ps->maxF, ps->nfeat_dev + cand, ps->desc + (size_t)q * F * 64, ps->nfeat_dev + q, ps->maxF, RATIO,
+                         ps->best, ps->d1, ps->d2, ps->pass, 0, s))) return r;
+    std::vector<float> kq((size_t)nq * 6), kc((size_t)nc * 6), xq((size_t)nq * 3), xc((size_t)nc * 3);
+    std::vector<int> best((size_t)nc); std::vector<float> d1((size_t)nc); std::vector<unsigned char> pass((size_t)nc);
+    KT_CUDA(cudaMemcpyAsync(kq.data(), ps->kp + (size_t)q * F * 6, kq.size() * 4, cudaMemcpyDeviceToHost, s));
+    KT_CUDA(cudaMemcpyAsync(kc.data(), ps->kp + (size_t)cand * F * 6, kc.size() * 4, cudaMemcpyDeviceToHost, s));
+    KT_CUDA(cudaMemcpyAsync(xq.data(), ps->xyz + (size_t)q * F * 3, xq.size() * 4, cudaMemcpyDeviceToHost, s));
+    KT_CUDA(cudaMemcpyAsync(xc.data(), ps->xyz + (size_t)cand * F * 3, xc.size() * 4, cudaMemcpyDeviceToHost, s));
+    KT_CUDA(cudaMemcpyAsync(best.data(), ps->best, best.size() * 4, cudaMemcpyDeviceToHost, s));
+    KT_CUDA(cudaMemcpyAsync(d1.data(), ps->d1, d1.size() * 4, cudaMemcpyDeviceToHost, s));
+    KT_CUDA(cudaMemcpyAsync(pass.data(), ps->pass, pass.size(), cudaMemcpyDeviceToHost, s));
+    KT_CUDA(cudaStreamSynchronize(s));
+    std::vector<int> oi, ni;
+    place_match_3d(best.data(), d1.data(), pass.data(), nc, nq, xc.data(), xq.data(), oi, ni);
+    const int m = (int)oi.size();
+    res->matches = m; res->stage = KT_PLACE_MATCHES;
+    if (m < MIN_MATCHES) return 0;
+    // PnP RANSAC: new 3-D points, old keypoints (PNPSolver.cpp:51-75)
+    std::vector<float> pn((size_t)m * 3), po((size_t)m * 3), uv((size_t)m * 2), kpn((size_t)m * 2), kpo((size_t)m * 2);
+    for (int k = 0; k < m; ++k) {
+        const int a = ni[k], b = oi[k];
+        for (int e = 0; e < 3; ++e) { pn[(size_t)k * 3 + e] = xq[(size_t)a * 3 + e]; po[(size_t)k * 3 + e] = xc[(size_t)b * 3 + e]; }
+        uv[(size_t)k * 2] = kc[(size_t)b * 6]; uv[(size_t)k * 2 + 1] = kc[(size_t)b * 6 + 1];
+        kpn[(size_t)k * 2] = kq[(size_t)a * 6]; kpn[(size_t)k * 2 + 1] = kq[(size_t)a * 6 + 1]; kpo[(size_t)k * 2] = uv[(size_t)k * 2]; kpo[(size_t)k * 2 + 1] = uv[(size_t)k * 2 + 1];
+    }
+    KT_CUDA(cudaMemcpyAsync(ps->pn, pn.data(), pn.size() * 4, cudaMemcpyHostToDevice, s));
+    KT_CUDA(cudaMemcpyAsync(ps->po, po.data(), po.size() * 4, cudaMemcpyHostToDevice, s));
+    KT_CUDA(cudaMemcpyAsync(ps->uv, uv.data(), uv.size() * 4, cudaMemcpyHostToDevice, s));
+    PnpArgs pa; pa.p_new = ps->pn; pa.p_old = ps->po; pa.uv_old = ps->uv; pa.n = m; pa.k = K; pa.iterations = PNP_ITERS; pa.threshold_px = 2.f;
+    pa.seed = 0x4b696e74756f7573ull;
+    if ((r = pnp_ransac(pa, &ps->pnp_ws, ps->pose, ps->inl, ps->ninl, s))) return r;
+    double pose12[12]; int n_in = 0; std::vector<unsigned char> inl((size_t)m);
+    KT_CUDA(cudaMemcpyAsync(pose12, ps->pose, sizeof(pose12), cudaMemcpyDeviceToHost, s));
+    KT_CUDA(cudaMemcpyAsync(&n_in, ps->ninl, sizeof(int), cudaMemcpyDeviceToHost, s));
+    KT_CUDA(cudaMemcpyAsync(inl.data(), ps->inl, inl.size(), cudaMemcpyDeviceToHost, s));
+    KT_CUDA(cudaStreamSynchronize(s));
+    res->inliers = n_in; res->inlier_ratio = (float)n_in / (float)m; res->stage = KT_PLACE_INLIERS;
+    if (!((float)n_in / (float)m > ps->p.inlier_ratio)) return 0;
+    // dense check: both keyframes' maps by the fused front end, the new one moved into the old camera by the PnP pose, then the tracker's
+    // whole-frame projective ICP with the old keyframe's maps as the model (camera at the identity)
+    double Tp[16]; m4_from12(pose12, Tp);
+    for (int sidx = 0; sidx < 2; ++sidx) {
+        const uint16_t* dk = ps->depth + (size_t)(sidx == 0 ? cand : q) * P;
+        if ((r = bilateral_scale(dk, ps->depths[sidx][0], 0, ps->rows, ps->cols, K, false, s))) return r;
+        FrontendArgs fa; std::memset(&fa, 0, sizeof(fa));
+        fa.depth_f = ps->depths[sidx][0]; fa.depth_raw = dk; fa.rows = ps->rows; fa.cols = ps->cols; fa.k = K;
+        fa.depths = ps->depths[sidx]; fa.vmaps = ps->vmaps[sidx]; fa.nmaps = ps->nmaps[sidx];
+        if ((r = frontend_pyramid(fa, s))) return r;
+    }
+    float Rp[9], tp[3];
+    for (int i = 0; i < 3; ++i) { for (int j = 0; j < 3; ++j) Rp[i * 3 + j] = (float)Tp[i * 4 + j]; tp[i] = (float)Tp[i * 4 + 3]; }
+    TransformLevel tl[LEVELS];
+    for (int l = 0; l < LEVELS; ++l) { tl[l].vs = ps->vmaps[1][l]; tl[l].ns = ps->nmaps[1][l]; tl[l].vd = ps->vmaps[1][l]; tl[l].nd = ps->nmaps[1][l]; tl[l].rows = ps->rows >> l; tl[l].cols = ps->cols >> l; }
+    if ((r = transform_maps_pyramid(tl, LEVELS, to_mat33(Rp), make_float3(tp[0], tp[1], tp[2]), s))) return r;
+    const float* vc4[LEVELS]; const float* nc4[LEVELS]; const float* vm4[LEVELS]; const float* nm4[LEVELS];
+    for (int l = 0; l < LEVELS; ++l) { vc4[l] = ps->vmaps[1][l]; nc4[l] = ps->nmaps[1][l]; vm4[l] = ps->vmaps[0][l]; nm4[l] = ps->nmaps[0][l]; }
+    const OdomMaps maps = {vc4, nc4, vm4, nm4};
+    IcpLevelArgs la[LEVELS]; RgbLevelArgs ra[LEVELS];
+    for (int l = 0; l < LEVELS; ++l) odom_level_args(c, maps, l, &la[l], &ra[l]);
+    const float pose_id[12] = {1, 0, 0, 0, 1, 0, 0, 0, 1, 0, 0, 0};
+    if ((r = odom_exchange_reset(ps->xwords, s))) return r;
+    if ((r = icp_frame(la, c->iterations, pose_id, ps->state, ps->xwords, ps->trace, &ps->state->odo_timeout, 0, 0, 0, s))) return r;
+    float Rt[13];
+    KT_CUDA(cudaMemcpyAsync(Rt, (char*)ps->state + offsetof(OdomState, Rcurr), 13 * sizeof(float), cudaMemcpyDeviceToHost, s));
+    KT_CUDA(cudaStreamSynchronize(s));
+    if (((int*)Rt)[12]) { set_error("kt_detect_loops: the ICP kernel's grid-wide sum gave up"); return KT_ERR_STATE; }
+    double dT[16], T[16], C[16];
+    for (int i = 0; i < 3; ++i) { for (int j = 0; j < 3; ++j) dT[i * 4 + j] = Rt[i * 3 + j]; dT[i * 4 + 3] = Rt[9 + i]; }
+    dT[12] = dT[13] = dT[14] = 0; dT[15] = 1;
+    m4_mul(dT, Tp, T);                 // new camera -> old camera
+    m4_rigid_inverse(T, C);            // old -> new: the pose of the old camera in the new one (icpDepthFrames' result)
+    // fitness: the old keyframe's cloud moved by C against the new one's, both at 2.5 voxels (PlaceRecognition.cpp:238-276)
+    if ((r = depth_to_cloud(ps->depth + (size_t)cand * P, ps->rows, ps->cols, K, ps->cloud[0], s))) return r;
+    if ((r = depth_to_cloud(ps->depth + (size_t)q * P, ps->rows, ps->cols, K, ps->cloud[1], s))) return r;
+    float T12[12];
+    for (int i = 0; i < 3; ++i) for (int j = 0; j < 4; ++j) T12[i * 4 + j] = (float)C[i * 4 + j];
+    size_t ns = 0, nd = 0;
+    if ((r = cloud_fitness(ps->cloud[0], P, ps->cloud[1], P, 2.5f * c->voxel, T12, &ps->ws[0], &ps->ws[1], ps->cent[0], ps->cent[1], P, ps->d2fit, &res->fitness, &ns, &nd, s))) return r;
+    res->stage = KT_PLACE_FITNESS;
+    if (!(res->fitness >= 0.0 && res->fitness < 0.01)) return 0;
+    // the loop: inliers back-projected at their truncated pixels (DepthCamera::projectInlierMatches)
+    std::vector<uint16_t> hd_new(P), hd_old(P);
+    KT_CUDA(cudaMemcpyAsync(hd_new.data(), ps->depth + (size_t)q * P, P * 2, cudaMemcpyDeviceToHost, s));
+    KT_CUDA(cudaMemcpyAsync(hd_old.data(), ps->depth + (size_t)cand * P, P * 2, cudaMemcpyDeviceToHost, s));
+    KT_CUDA(cudaStreamSynchronize(s));
+    ps->in_new.emplace_back(); ps->in_old.emplace_back();
+    std::vector<float>& a1 = ps->in_new.back(); std::vector<float>& a2 = ps->in_old.back();
+    place_project_inliers(kpn.data(), kpo.data(), inl.data(), m, hd_new.data(), hd_old.data(), ps->rows, ps->cols, intr, a1, a2);
+    res->stage = KT_PLACE_LOOP;
+    res->constraint.time1 = res->time; res->constraint.time2 = res->candidate_time;
+    for (int k = 0; k < 16; ++k) res->constraint.constraint[k] = C[k];
+    res->constraint.n_inliers = a1.size() / 3;
+    res->constraint.inliers1 = a1.empty() ? 0 : a1.data(); res->constraint.inliers2 = a2.empty() ? 0 : a2.data();
+    return 0;
+}
+
+} // namespace
+
+int kt_detect_loops(kt_ctx* c, kt_place_result* out, size_t capacity, size_t* n_out)
+{
+    if (n_out) *n_out = 0;
+    if (!c || (!out && capacity)) { set_error("kt_detect_loops: bad argument"); return KT_ERR_INVALID; }
+    if (c->world > 1) { set_error("kt_detect_loops: a volume shared by %d GPUs has no loop detection", c->world); return KT_ERR_INVALID; }
+    if (!c->place) { set_error("kt_detect_loops: loop detection is off (kt_set_loop_detection)"); return KT_ERR_STATE; }
+    KT_CUDA(cudaSetDevice(c->cfg.device));
+    PlaceStore* ps = c->place;
+    KT_CUDA(cudaStreamSynchronize(ps->stream));                  // every capture has landed
+    ps->in_new.clear(); ps->in_old.clear();
+    const size_t pending = ps->times.size() - ps->processed;
+    ps->in_new.reserve(std::min(capacity, pending)); ps->in_old.reserve(std::min(capacity, pending));  // constraints point into these until the next call
+    size_t n = 0;
+    while (n < capacity && ps->processed < ps->times.size()) {
+        kt_place_result* res = &out[n];
+        int r = place_process(c, (int)ps->processed, res);
+        ++ps->processed; ++n;
+        if (n_out) *n_out = n;
+        if (r) return r;
+        if (res->stage == KT_PLACE_LOOP && ps->p.close) {
+            r = kt_close_loop(c, &res->constraint, ps->p.pose_spacing, ps->p.node_spacing, ps->p.isam_thresh, &res->report);
+            if (r) return r;
+            res->closed = res->report.accepted;
+        }
+        // the -lt throttle starts with a loop the backend ACCEPTS (Deformation.cpp:258-260 sets lastLoopTime after the iSAM gate); with
+        // close = 0 the library never learns the outcome, so it starts with every loop found
+        if (res->stage == KT_PLACE_LOOP && (!ps->p.close || res->closed)) ps->last_loop = res->time;
+    }
+    return KT_OK;
+}
+
 int kt_num_pose_graph_nodes(kt_ctx* c) { return c ? (int)c->pgo_nodes.size() : 0; }
 int kt_get_pose_graph_node(kt_ctx* c, int idx, kt_dense_pose* out)
 {

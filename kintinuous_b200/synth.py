@@ -50,10 +50,25 @@ def _texture(p):
     return np.clip(np.rint(out), 0, 255).astype(np.uint8)
 
 
+def cell_texture(p, cell: float = 0.05):
+    """Opt-in aperiodic texture (render_at's `texture`): cells of the world grid `cell` metres wide, each a grey level drawn from a hash of
+    the cell's integer coordinates.  The default texture's checker repeats every 15.7 cm, so most SURF features there have look-alikes."""
+    i = np.floor(p / cell).astype(np.int64)
+    h = (((i[..., 0] * 73856093) ^ (i[..., 1] * 19349663) ^ (i[..., 2] * 83492791)) * 0x45D9F3B) & 0xFFFFFFFF
+    return np.repeat(np.rint((((h >> 16) ^ h) & 0xFFFF) * (255.0 / 65535.0))[..., None], 3, -1).astype(np.uint8)
+
+
 def render(k: int, cols: int = 640, rows: int = 480, noise: bool = False):
-    """Returns (depth uint16 [rows, cols] in mm, rgb uint8 [rows, cols, 3])."""
-    fx, fy, cx, cy = intrinsics(cols, rows)
+    """Returns (depth uint16 [rows, cols] in mm, rgb uint8 [rows, cols, 3]) of frame k of the default trajectory."""
     R, t = pose(k)
+    return render_at(R, t, cols, rows, noise, noise_seed=k)
+
+
+def render_at(R, t, cols: int = 640, rows: int = 480, noise: bool = False, noise_seed: int = 0, texture=None):
+    """The scene seen by a camera at any pose (R, t camera -> world); the axial noise draws from default_rng(SEED + noise_seed).
+    texture: optional replacement of the default texture function (world points [..., 3] -> uint8 RGB [..., 3])."""
+    fx, fy, cx, cy = intrinsics(cols, rows)
+    R = np.asarray(R, np.float64); t = np.asarray(t, np.float64)
     u, v = np.meshgrid(np.arange(cols, dtype=np.float64), np.arange(rows, dtype=np.float64))
     dc = np.stack([(u - cx) / fx, (v - cy) / fy, np.ones_like(u)], axis=-1)       # camera-frame ray, z = 1
     d = dc @ R.T                                                                  # world direction (not normalised)
@@ -81,9 +96,9 @@ def render(k: int, cols: int = 640, rows: int = 480, noise: bool = False):
     # with a z = 1 camera ray, the ray parameter IS the camera-frame depth
     z = t_hit
     p = o + d * t_hit[..., None]
-    rgb = _texture(p)
+    rgb = (texture or _texture)(p)
     if noise:
-        rng = np.random.default_rng(SEED + k)
+        rng = np.random.default_rng(SEED + noise_seed)
         sigma = 0.0012 + 0.0019 * (z - 0.4) ** 2
         z = z + rng.standard_normal(z.shape) * sigma
     mm = np.rint(1000.0 * z)
