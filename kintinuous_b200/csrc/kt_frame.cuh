@@ -179,19 +179,27 @@ __device__ __forceinline__ void mbar_wait(unsigned long long* bar, unsigned int 
         "}\n" :: "r"(smem_u32(bar)), "r"(parity) : "memory");
 }
 
-// 32 per-lane values -> lane l holds the warp total of value l (31 shuffles instead of 32 x 5; fixed tree)
+// 32 per-lane values -> lane l holds the warp total of value l (31 shuffles instead of 32 x 5; fixed tree).  One template instance per
+// step, so that every index into v is a compile-time constant: with the step as a loop variable nvcc leaves the loop rolled in the
+// whole-frame kernels, which puts v -- the thread's running sums, updated for every pixel -- in local memory (DESIGN.md section 3.2).
+template <int STEP>
+__device__ __forceinline__ void warp_transpose_step(float (&v)[32], int lane)
+{
+    const bool upper = (lane & STEP) != 0;
+#pragma unroll
+    for (int j = 0; j < STEP; ++j) {
+        const float send = upper ? v[j] : v[j + STEP];
+        const float keep = upper ? v[j + STEP] : v[j];
+        v[j] = keep + __shfl_xor_sync(0xffffffffu, send, STEP);
+    }
+}
 __device__ __forceinline__ float warp_transpose_sum(float (&v)[32], int lane)
 {
-#pragma unroll
-    for (int step = 16; step >= 1; step >>= 1) {
-        const bool upper = (lane & step) != 0;
-#pragma unroll
-        for (int j = 0; j < step; ++j) {
-            const float send = upper ? v[j] : v[j + step];
-            const float keep = upper ? v[j + step] : v[j];
-            v[j] = keep + __shfl_xor_sync(0xffffffffu, send, step);
-        }
-    }
+    warp_transpose_step<16>(v, lane);
+    warp_transpose_step<8>(v, lane);
+    warp_transpose_step<4>(v, lane);
+    warp_transpose_step<2>(v, lane);
+    warp_transpose_step<1>(v, lane);
     return v[0];
 }
 
