@@ -200,6 +200,35 @@ KT_API int kt_get_deformed_slice_mesh(kt_ctx* ctx, int idx, kt_mesh_vertex* vert
 /* The "_opt" mesh of Deformation::saveMesh (Deformation.cpp:85-100): kt_save_mesh_ply's layout over the deformed vertices of the slices
  * covered by the last kt_deform_map.  KT_ERR_STATE before any kt_deform_map or when none of those slices has a mesh. */
 KT_API int kt_save_deformed_mesh_ply(kt_ctx* ctx, const char* path);
+/* The map as one point cloud: the files a run exists to produce (MainController.cpp:238-265).
+ *   which = 0, the recorded map (CloudSliceProcessor::save, CloudSliceProcessor.cpp:180-231): the processed cloud of every slice recorded
+ *     with slice processing on since the last reset, in order, the FINAL slice of kt_finalise included.
+ *   which = 1, the corrected map (Deformation::saveCloud, Deformation.cpp:67-83): the slices covered by the last kt_deform_map /
+ *     kt_close_loop contribute their deformed copies (kt_get_deformed_slice); every slice recorded after it is moved rigidly by that
+ *     deformation's last correction C = P_corr(t) P_tracked(t)^-1, with t the last corrected pose passed to kt_deform_map (the identity
+ *     when it was given point constraints only) or the last pose-graph node of kt_close_loop -- what iSAM's odometry chain gives a pose
+ *     after the last loop (Deformation::addVertices, :421-457).  Positions x' = R x + t and normals n' = R n in FP32 on the device (the
+ *     reference's pcl::transformPointCloud leaves the normals unrotated).  KT_ERR_STATE before any deformation or after kt_reset.
+ *   dedupe = 1 is the reference's -nos: pcl::VoxelGrid at kt_get_voxel_size over the whole concatenation (kt_op_voxel_grid), which merges
+ *     the points that neighbouring slices repeat in their overlap planes.  Without it the recorded map is copied on the host, no GPU work.
+ * kt_get_map_cloud copies up to `capacity` points (out may be NULL: the count alone) and returns the full count; every call redoes the
+ * work, so a count-then-fetch pair costs two exports.  It waits for slice downloads still in flight and works on the slice stream
+ * between frames: tracking reads nothing it writes.  kt_save_map_pcd writes the same cloud as PCL 1.7.2's savePCDFile(path, cloud, true):
+ * the ASCII header (FIELDS x y z rgb normal_x normal_y normal_z curvature, DATA binary), then 32 packed little-endian bytes per point in
+ * field order (rgb = the b, g, r, a bytes).  The reference's files: "<log>.pcd" = (which 0, dedupe -nos), "<log>_opt.pcd" = (which 1,
+ * dedupe 0).  KT_ERR_STATE when no slice was recorded with slice processing on; KT_ERR_INVALID for a volume shared by several GPUs
+ * (world > 1: each rank's slices hold only its own voxels); KT_ERR_CUDA when device memory for the export cannot be allocated (nothing
+ * else changes). */
+typedef struct kt_map_report {
+    size_t input_points;        /* points of the concatenation */
+    size_t output_points;       /* points of the exported cloud (the voxel grid's leaves with dedupe) */
+    int slices;                 /* slices recorded with slice processing on */
+    int moved_slices;           /* slices placed by the rigid correction (which = 1) */
+    int pcl_would_skip;         /* dedupe: PCL's int64 check fired, so PCL would have returned the cloud unfiltered (this export filters) */
+    float upload_ms, sort_ms, centroid_ms, download_ms, total_ms;   /* CUDA-event times of the device work (0 without any) */
+} kt_map_report;
+KT_API int kt_get_map_cloud(kt_ctx* ctx, int which, int dedupe, kt_point_xyzrgbnormal* out, size_t capacity, size_t* count, kt_map_report* report);
+KT_API int kt_save_map_pcd(kt_ctx* ctx, const char* path, int which, int dedupe, kt_map_report* report);
 /* Loop closure: the pose-graph half of the reference's backend (backend/Deformation.cpp:130-346 addCameraCamera / addCameraLoop,
  * backend/iSAMInterface.cpp) on the GPU.  The caller passes what PlaceRecognition produces (LoopClosureConstraint,
  * PlaceRecognition.cpp:198-209): time1 (the new frame) and time2 (the old one), both dense pose timestamps, the pose of the camera at
@@ -407,6 +436,14 @@ KT_API int kt_op_extract_slice(const int16_t* tsdf_dev, const float* volume_size
  * filter in that case). */
 KT_API int kt_op_process_slice(const kt_point_xyzrgb* points_dev, size_t n, int weight_cull, float leaf, int k_search,
                                kt_point_xyzrgbnormal* out_dev, size_t capacity, size_t* count, void* stream);
+/* pcl::VoxelGrid<PointT>::applyFilter (PCL 1.7.2, downsample_all_data, kt_map.cu) over n device points of kind 0 (kt_point_xyzrgb) or
+ * 1 (kt_point_xyzrgbnormal): one centroid per occupied leaf of edge `leaf`, in ascending leaf index, every field averaged in PCL's float
+ * arithmetic (points of a leaf added in input order, from the first point on), colour truncated, alpha 0.  Writes up to `capacity`
+ * points of the same kind to out_dev and returns the full count.  Leaf indices are 64-bit: where PCL's int64 check finds more than
+ * INT_MAX cells, PCL returns the cloud unfiltered; this filters and sets *pcl_would_skip = 1.  KT_ERR_INVALID for a non-finite x / y / z,
+ * more than 2^62 cells or 2^31 - 1 points; KT_ERR_CUDA when its scratch cannot be allocated. */
+KT_API int kt_op_voxel_grid(const void* points_dev, size_t n, int kind, float leaf, void* out_dev, size_t capacity, size_t* count,
+                            int* pcl_would_skip, void* stream);
 /* Marching cubes over the cells of the logical box [minX,maxX) x [minY,maxY) x [minZ,maxZ) of the cyclic volume, with extractCloudSlice's
  * addressing (voxel_wrap3: storage offset, any value, reduced mod vol; real_voxel_wrap3: global offset of the positions).  Stands in
  * for calculateMesh (backend/MeshGenerator.cpp:193-227; a different algorithm, no parity with PCL's greedy projection).  A corner is

@@ -146,6 +146,16 @@ PGO_FACTOR_DTYPE = np.dtype([("i", "<i4"), ("j", "<i4"), ("z", "<f8", (6,))])
 assert PGO_FACTOR_DTYPE.itemsize == 56
 
 
+class MapReport(C.Structure):
+    """kt_map_report of kt_get_map_cloud / kt_save_map_pcd."""
+    _fields_ = [("input_points", C.c_size_t), ("output_points", C.c_size_t), ("slices", C.c_int), ("moved_slices", C.c_int),
+                ("pcl_would_skip", C.c_int), ("upload_ms", C.c_float), ("sort_ms", C.c_float), ("centroid_ms", C.c_float),
+                ("download_ms", C.c_float), ("total_ms", C.c_float)]
+
+    def as_dict(self):
+        return {k: getattr(self, k) for k, _ in self._fields_}
+
+
 class SliceInfo(C.Structure):
     _fields_ = [("dimension", C.c_int), ("odometry", C.c_int), ("camera_t", C.c_float * 3), ("camera_R", C.c_float * 9),
                 ("utime", C.c_uint64), ("count", C.c_size_t)]
@@ -339,6 +349,24 @@ class Tracker:
     def save_deformed_mesh_ply(self, path):
         """The deformed slice meshes of the last deform_map as one binary PLY (kt_save_deformed_mesh_ply)."""
         _check(self.lib.kt_save_deformed_mesh_ply(self.h, os.fsencode(path)))
+
+    def map_cloud(self, which=0, dedupe=False):
+        """The map as one cloud (kt_get_map_cloud): which 0 = the recorded map, 1 = the corrected map; dedupe = the reference's -nos
+        voxel grid over the concatenation.  Returns (POINT_NORMAL_DTYPE array, report dict).  Counts first, then fetches: with dedupe or
+        which = 1 that runs the export twice."""
+        n = C.c_size_t(0); rep = MapReport()
+        _check(self.lib.kt_get_map_cloud(self.h, int(which), int(dedupe), None, C.c_size_t(0), C.byref(n), C.byref(rep)))
+        pts = np.zeros(n.value, dtype=POINT_NORMAL_DTYPE)
+        if n.value:
+            _check(self.lib.kt_get_map_cloud(self.h, int(which), int(dedupe), _ptr(pts), C.c_size_t(n.value), C.byref(n), C.byref(rep)))
+        return pts[:n.value], rep.as_dict()
+
+    def save_map_pcd(self, path, which=0, dedupe=False):
+        """The same cloud as a binary .pcd (kt_save_map_pcd): the reference's <log>.pcd is which 0 with its -nos as dedupe, <log>_opt.pcd
+        is which 1 without.  Returns the report dict."""
+        rep = MapReport()
+        _check(self.lib.kt_save_map_pcd(self.h, os.fsencode(path), int(which), int(dedupe), C.byref(rep)))
+        return rep.as_dict()
 
     def close_loop(self, time1, time2, T, inliers1=None, inliers2=None, pose_spacing=0.0, node_spacing=0.8, isam_thresh=10.0):
         """Close a loop (kt_close_loop): T = pose of the camera at time2 in the frame of the camera at time1 (4 x 4); inliers1 / inliers2:
@@ -583,6 +611,14 @@ class _Ops:
         _check(self._l().kt_op_process_slice(_ptr(points_dev), C.c_size_t(n), int(weight_cull), C.c_float(leaf), int(k_search), _ptr(out_dev), C.c_size_t(capacity),
                                              C.byref(cnt), None))
         return cnt.value
+
+    def voxel_grid(self, points_dev, n, kind, leaf, out_dev, capacity):
+        """kt_op_voxel_grid: pcl::VoxelGrid over n device records of kind 0 (POINT_DTYPE) / 1 (POINT_NORMAL_DTYPE) into out_dev (up to
+        capacity records of the same kind).  Returns (leaves, pcl_would_skip)."""
+        cnt = C.c_size_t(0); skip = C.c_int(0)
+        _check(self._l().kt_op_voxel_grid(_ptr(points_dev), C.c_size_t(n), int(kind), C.c_float(leaf), _ptr(out_dev), C.c_size_t(capacity),
+                                          C.byref(cnt), C.byref(skip), None))
+        return cnt.value, skip.value
 
     def mesh_volume_into(self, tsdf, color, vol, volume_size, wrap, real_wrap, box, weight_cull, verts_dev, max_verts, tris_dev, max_tris):
         """kt_op_mesh_volume into caller buffers: (status, n_verts, n_tris); status is 0 or KT_ERR_CAPACITY (nothing written)."""

@@ -182,6 +182,12 @@ int kt_op_process_slice(const kt_point_xyzrgb* points_dev, size_t n, int weight_
     return process_slice(points_dev, n, weight_cull, leaf, k_search, out_dev, capacity, count, &g_ops.slice_ws, st(s));
 }
 
+int kt_op_voxel_grid(const void* points_dev, size_t n, int kind, float leaf, void* out_dev, size_t capacity, size_t* count, int* pcl_would_skip, void* s)
+{
+    if (!count || !pcl_would_skip || (capacity && !out_dev)) { set_error("kt_op_voxel_grid: bad argument"); return KT_ERR_INVALID; }
+    return voxel_grid(points_dev, n, kind, leaf, out_dev, capacity, count, pcl_would_skip, 0, st(s));
+}
+
 int kt_op_mesh_volume(const int16_t* tsdf, const uint8_t* color, int vol, const float* vs, const int* wrap, const int* real_wrap,
                       int minX, int maxX, int minY, int maxY, int minZ, int maxZ, int weight_cull, kt_mesh_vertex* verts, size_t max_verts,
                       uint32_t* tris, size_t max_tris, size_t* n_verts, size_t* n_tris, void* s)

@@ -229,6 +229,16 @@ int depth_to_cloud(const uint16_t* depth, int rows, int cols, const Intr& k, voi
 // getFitnessScore of the loop check: d2_dev holds capacity + 8 doubles; synchronises s
 int cloud_fitness(const void* src, size_t n_src, const void* dst, size_t n_dst, float leaf, const float* T12, SliceWorkspace* ws_src, SliceWorkspace* ws_dst,
                   void* src_out, void* dst_out, size_t capacity, double* d2_dev, double* fitness, size_t* n_src_used, size_t* n_dst_used, cudaStream_t s);
+// ---- whole-map export (kt_map.cu) ----
+// pcl::VoxelGrid (downsample_all_data) over n records of kind 0 (kt_point_xyzrgb) or 1 (kt_point_xyzrgbnormal): one centroid per leaf in
+// ascending 64-bit leaf index, the first min(leaves, capacity) written to out (may be null), *count = leaves; *pcl_would_skip = PCL's
+// int64 overflow check fired (PCL would return the input unfiltered).  ms2 (may be null): device ms of keys + sort, of leaf starts +
+// centroids.  Workspace allocated and freed per call; synchronises s.
+int voxel_grid(const void* points_dev, size_t n, int kind, float leaf, void* out_dev, size_t capacity, size_t* count, int* pcl_would_skip,
+               float* ms2, cudaStream_t s);
+struct RigidF { float R[9]; float t[3]; };       // row-major rotation and translation
+// x' = R x + t and n' = R n of n kt_point_xyzrgbnormal records in place, FP32 without contraction; asynchronous
+int rigid_move(void* points_dev, size_t n, const RigidF& C, cudaStream_t s);
 // cross-GPU barrier: every rank writes `epoch` into slot [rank] of every peer's flag array, then waits until all slots of its own
 // array reach `epoch` (bounded spin: returns through *error_dev != 0 instead of hanging the GPU if a peer never arrives)
 int xgpu_barrier(unsigned int* const* peer_flags_dev /* [world] device array of pointers */, unsigned int* my_flags, int rank, int world,

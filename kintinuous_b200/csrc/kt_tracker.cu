@@ -201,6 +201,10 @@ struct kt_ctx {
     // loop closure (kt_close_loop, kt_pgo.cu): the accepted loops with their inliers, and the optimised nodes of the last accepted one
     struct Loop { uint64_t time1, time2; double C[16]; std::vector<float> in1, in2; };
     std::vector<Loop> loops; std::vector<kt_dense_pose> pgo_nodes;
+    // the last correction of that deformation (kt_get_map_cloud's corrected map moves later slices by P_corr P_tracked^-1): the pose at
+    // `time` as tracked and as corrected (the last corrected pose of kt_deform_map, the last pose-graph node of kt_close_loop)
+    struct MapCorrection { uint64_t time; float tracked[16]; float corrected[16]; };
+    MapCorrection map_corr;
     // RGB-D
     float* lastDepth[LEVELS]; float* nextDepth[LEVELS]; uint8_t* lastImage[LEVELS]; uint8_t* nextImage[LEVELS];
     int16_t* nextdIdx[LEVELS]; int16_t* nextdIdy[LEVELS]; float* pointClouds[LEVELS]; void* corresImg[LEVELS];
@@ -718,6 +722,7 @@ int kt_reset(kt_ctx* c)
     c->deformed.clear();
     if (c->deform_arena) c->deform_arena->rewind();
     c->loops.clear(); c->pgo_nodes.clear();
+    std::memset(&c->map_corr, 0, sizeof(c->map_corr));
     if (c->place) {                              // reset(): the place-recognition buffer starts again (.cpp:290-298)
         cudaStreamSynchronize(c->place->stream);
         c->place->times.clear(); c->place->dense_idx.clear(); c->place->processed = 0; c->place->full = false; c->place->last_loop = 0;
@@ -1315,7 +1320,20 @@ int kt_deform_map(kt_ctx* c, const kt_dense_pose* corrected, size_t n, const kt_
             else set_error("kt_deform_map: point constraint %zu has a source or target that is not finite", l - n);
             return KT_ERR_INVALID;
         }
-    return deform_run(c, npos, ntime, cons, report);
+    r = deform_run(c, npos, ntime, cons, report);
+    if (r) return r;
+    // the correction later slices follow: the last corrected pose and the dense pose it corrects (the last one with its timestamp,
+    // as iSAM's camera map keeps it); point constraints alone correct no pose
+    kt_ctx::MapCorrection mc; std::memset(&mc, 0, sizeof(mc));
+    for (int e = 0; e < 4; ++e) mc.tracked[5 * e] = mc.corrected[5 * e] = 1.f;
+    if (n) {
+        mc.time = corrected[n - 1].timestamp;
+        std::memcpy(mc.corrected, corrected[n - 1].pose, sizeof(mc.corrected));
+        for (size_t i = nd; i-- > 0;)
+            if (c->dense_poses[i].timestamp == mc.time) { std::memcpy(mc.tracked, c->dense_poses[i].pose, sizeof(mc.tracked)); break; }
+    }
+    c->map_corr = mc;
+    return KT_OK;
 }
 
 // Deformation::addCameraCamera + addCameraLoop (Deformation.cpp:130-346) with iSAMInterface (iSAMInterface.cpp:44-140): the pose graph of
@@ -1425,6 +1443,9 @@ int kt_close_loop(kt_ctx* c, const kt_loop_constraint* loop, float pose_spacing,
         r = deform_run(c, npos, ntime, cons, &report->deform);
         if (r) return r;
         report->map_deformed = report->deform.deformed;
+        c->map_corr.time = nodes[n - 1].timestamp;
+        std::memcpy(c->map_corr.tracked, c->dense_poses[take[n - 1]].pose, sizeof(c->map_corr.tracked));
+        std::memcpy(c->map_corr.corrected, nodes[n - 1].pose, sizeof(c->map_corr.corrected));
     }
     c->loops.swap(loops);
     c->pgo_nodes.swap(nodes);
@@ -1712,6 +1733,146 @@ int kt_save_deformed_mesh_ply(kt_ctx* c, const char* path)
     if (!c || !path) return KT_ERR_INVALID;
     if (c->deformed.empty()) { set_error("kt_save_deformed_mesh_ply: no kt_deform_map since the last reset"); return KT_ERR_STATE; }
     return save_mesh_ply(c, path, c->deformed.size(), true, "kt_save_deformed_mesh_ply");
+}
+
+// The map as one cloud (kt_get_map_cloud, kt_save_map_pcd; the header describes which / dedupe).  The points go to out (up to capacity),
+// or, with `grow`, to a host vector sized to the full count.  Device work, if any, runs on the slice stream with scratch that is freed
+// before returning; nothing the tracker reads is written.
+static int map_cloud(kt_ctx* c, int which, int dedupe, kt_point_xyzrgbnormal* out, size_t capacity, std::vector<kt_point_xyzrgbnormal>* grow,
+                     size_t* count, kt_map_report* report, const char* who)
+{
+    kt_map_report R; std::memset(&R, 0, sizeof(R));
+    if (report) *report = R;
+    if (count) *count = 0;
+    if (which != 0 && which != 1) { set_error("%s: which must be 0 (recorded map) or 1 (corrected map)", who); return KT_ERR_INVALID; }
+    if (c->world > 1) { set_error("%s: each of the %d GPUs sharing the volume holds only its own voxels of a slice", who, c->world); return KT_ERR_INVALID; }
+    KT_CUDA(cudaSetDevice(c->cfg.device));
+    if (c->stream_slices) KT_CUDA(cudaStreamSynchronize(c->stream_slices));           // every slice has landed in its pinned buffers
+    // slices [0, covered) come from the deformed copies; with which = 1 the later ones are moved rigidly and follow them
+    const size_t covered = which == 1 ? c->deformed.size() : c->slices.size();
+    size_t n = 0, n_fixed = 0;
+    for (size_t i = 0; i < c->slices.size(); ++i) {
+        const SliceRec& s = c->slices[i];
+        if (!s.has_processed) continue;
+        ++R.slices; n += s.processed_count;
+        if (i < covered) n_fixed += s.processed_count; else ++R.moved_slices;
+    }
+    if (!R.slices) { set_error("%s: no slice was recorded with slice processing on (kt_set_slice_processing)", who); return KT_ERR_STATE; }
+    if (which == 1 && c->deformed.empty()) { set_error("%s: no kt_deform_map / kt_close_loop has deformed the map since the last reset", who); return KT_ERR_STATE; }
+    auto src = [&](size_t i) -> const kt_point_xyzrgbnormal* { return which == 1 && i < covered ? c->deformed[i].processed : c->slices[i].processed; };
+    const size_t rec = sizeof(kt_point_xyzrgbnormal);
+    R.input_points = n;
+    if (!dedupe && n_fixed == n) {                                                     // a concatenation of pinned host buffers
+        R.output_points = n;
+        if (grow) { grow->resize(n); out = grow->data(); capacity = n; }
+        size_t off = 0;
+        for (size_t i = 0; i < c->slices.size() && out && off < capacity; ++i) {
+            const SliceRec& s = c->slices[i];
+            if (!s.has_processed || !s.processed_count) continue;
+            const size_t k = std::min(s.processed_count, capacity - off);
+            std::memcpy(out + off, src(i), k * rec);
+            off += k;
+        }
+    } else if (n) {
+        cudaStream_t s = c->stream_slices;
+        void* d_in = 0; void* d_out = 0;
+        cudaEvent_t ev[4] = {0, 0, 0, 0};
+        auto run = [&]() -> int {
+            for (int e = 0; e < 4; ++e) KT_CUDA(cudaEventCreate(&ev[e]));
+            if (cudaMalloc(&d_in, n * rec) != cudaSuccess || (dedupe && cudaMalloc(&d_out, n * rec) != cudaSuccess)) {
+                cudaGetLastError();                                                    // not sticky: the next frame must not see it
+                set_error("%s: cannot allocate device memory for %zu points", who, n); return KT_ERR_CUDA;
+            }
+            KT_CUDA(cudaEventRecord(ev[0], s));
+            size_t off = 0;
+            for (size_t i = 0; i < c->slices.size(); ++i) {
+                const SliceRec& sl = c->slices[i];
+                if (!sl.has_processed || !sl.processed_count) continue;
+                KT_CUDA(cudaMemcpyAsync((char*)d_in + off * rec, src(i), sl.processed_count * rec, cudaMemcpyHostToDevice, s));
+                off += sl.processed_count;
+            }
+            KT_CUDA(cudaEventRecord(ev[1], s));
+            if (n_fixed < n) {
+                // C = P_corr(t) P_tracked(t)^-1 in FP64, the rigid inverse [R^T | -R^T t], rounded to float
+                const float* Pt = c->map_corr.tracked; const float* Pc = c->map_corr.corrected;
+                RigidF C;
+                for (int a = 0; a < 3; ++a) {
+                    for (int b = 0; b < 3; ++b) {
+                        double v = 0;
+                        for (int k = 0; k < 3; ++k) v += (double)Pc[4 * a + k] * (double)Pt[4 * b + k];
+                        C.R[3 * a + b] = (float)v;
+                    }
+                    double t = Pc[4 * a + 3];
+                    for (int b = 0; b < 3; ++b) {
+                        double v = 0;
+                        for (int k = 0; k < 3; ++k) v += (double)Pc[4 * a + k] * (double)Pt[4 * b + k];
+                        t -= v * (double)Pt[4 * b + 3];
+                    }
+                    C.t[a] = (float)t;
+                }
+                int r = rigid_move((kt_point_xyzrgbnormal*)d_in + n_fixed, n - n_fixed, C, s); if (r) return r;
+            }
+            size_t m = n;
+            float ms2[2] = {0.f, 0.f};
+            if (dedupe) { int r = voxel_grid(d_in, n, 1, c->voxel, d_out, n, &m, &R.pcl_would_skip, ms2, s); if (r) return r; }
+            R.output_points = m;
+            if (grow) { grow->resize(m); out = grow->data(); capacity = m; }
+            KT_CUDA(cudaEventRecord(ev[2], s));
+            const size_t k = out ? std::min(m, capacity) : 0;
+            if (k) KT_CUDA(cudaMemcpyAsync(out, dedupe ? d_out : d_in, k * rec, cudaMemcpyDeviceToHost, s));
+            KT_CUDA(cudaEventRecord(ev[3], s));
+            KT_CUDA(cudaStreamSynchronize(s));
+            KT_CUDA(cudaEventElapsedTime(&R.upload_ms, ev[0], ev[1]));
+            KT_CUDA(cudaEventElapsedTime(&R.download_ms, ev[2], ev[3]));
+            KT_CUDA(cudaEventElapsedTime(&R.total_ms, ev[0], ev[3]));
+            R.sort_ms = ms2[0]; R.centroid_ms = ms2[1];
+            return 0;
+        };
+        const int r = run();
+        cudaStreamSynchronize(s);
+        cudaFree(d_in); cudaFree(d_out);
+        for (int e = 0; e < 4; ++e) if (ev[e]) cudaEventDestroy(ev[e]);
+        if (r) return r;
+    }
+    if (count) *count = R.output_points;
+    if (report) *report = R;
+    return KT_OK;
+}
+
+int kt_get_map_cloud(kt_ctx* c, int which, int dedupe, kt_point_xyzrgbnormal* out, size_t capacity, size_t* count, kt_map_report* report)
+{
+    if (!c || !count) { set_error("kt_get_map_cloud: bad argument"); return KT_ERR_INVALID; }
+    return map_cloud(c, which, dedupe != 0, out, out ? capacity : 0, 0, count, report, "kt_get_map_cloud");
+}
+
+// PCL 1.7.2 PCDWriter::writeBinary of a PointXYZRGBNormal cloud (generateHeader, then the fields packed without padding)
+int kt_save_map_pcd(kt_ctx* c, const char* path, int which, int dedupe, kt_map_report* report)
+{
+    if (!c || !path) { set_error("kt_save_map_pcd: bad argument"); return KT_ERR_INVALID; }
+    std::vector<kt_point_xyzrgbnormal> cloud;
+    size_t n = 0;
+    int r = map_cloud(c, which, dedupe != 0, 0, 0, &cloud, &n, report, "kt_save_map_pcd"); if (r) return r;
+    FILE* f = fopen(path, "wb");
+    if (!f) { set_error("kt_save_map_pcd: cannot open %s", path); return KT_ERR_INVALID; }
+    fprintf(f, "# .PCD v0.7 - Point Cloud Data file format\nVERSION 0.7\nFIELDS x y z rgb normal_x normal_y normal_z curvature\n"
+               "SIZE 4 4 4 4 4 4 4 4\nTYPE F F F F F F F F\nCOUNT 1 1 1 1 1 1 1 1\nWIDTH %zu\nHEIGHT 1\nVIEWPOINT 0 0 0 1 0 0 0\n"
+               "POINTS %zu\nDATA binary\n", n, n);
+    std::vector<unsigned char> buf;
+    bool ok = true;
+    const size_t CH = 1 << 16;
+    for (size_t b = 0; b < n && ok; b += CH) {                     // x86 / aarch64 hosts are little-endian: the fields' raw bytes
+        const size_t k = std::min(CH, n - b);
+        buf.resize(k * 32);
+        for (size_t i = 0; i < k; ++i) {
+            const kt_point_xyzrgbnormal& p = cloud[b + i];
+            unsigned char* o = &buf[i * 32];
+            std::memcpy(o, &p.x, 12); std::memcpy(o + 12, &p.b, 4); std::memcpy(o + 16, &p.nx, 12); std::memcpy(o + 28, &p.curvature, 4);
+        }
+        ok = fwrite(buf.data(), 1, buf.size(), f) == buf.size();
+    }
+    if (fclose(f) != 0) ok = false;
+    if (!ok) { set_error("kt_save_map_pcd: writing %s failed", path); return KT_ERR_CUDA; }
+    return KT_OK;
 }
 
 int kt_get_slice_info(kt_ctx* c, int idx, kt_slice_info* info)
