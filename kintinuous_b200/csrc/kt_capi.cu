@@ -23,39 +23,40 @@ cudaStream_t st(void* s) { return (cudaStream_t)s; }
 // either: internal.h:299-536 has static state in computeDerivativeImages and __device__ globals in extract.cu).  One set PER DEVICE
 // (the device current at the call), and the calls that use it are serialised by a process-wide mutex, so operator calls from several
 // host threads / on several devices are safe, just not concurrent.
-struct OpScratch { OdomState* state; float* partials; int* ipartials; float* ztable; int ztable_n; unsigned int* counter; OdomState* host_state; SliceWorkspace slice_ws;
-                   MeshWorkspace mesh_ws; SurfWorkspace surf_ws; PnpWorkspace pnp_ws; SliceWorkspace fit_ws;
-                   int* place_ints; size_t place_ints_cap; };       // kt_op_surf / kt_op_match_ratio: counts in, counts out (grown on demand)
+struct OpScratch { Allocations mem; OdomState* state; float* partials; int* ipartials; unsigned int* counter; OdomState* host_state;
+                   DeviceBuffer<float> ztable; SliceWorkspace slice_ws; MeshWorkspace mesh_ws; SurfWorkspace surf_ws; PnpWorkspace pnp_ws;
+                   SliceWorkspace fit_ws; DeviceBuffer<int> place_ints; };   // place_ints: kt_op_surf / kt_op_match_ratio counts in, counts out
 enum { KT_MAX_DEVICES = 64 };
-OpScratch g_ops_dev[KT_MAX_DEVICES];
+// Allocated once per device and never destroyed: no CUDA call may run in the static destructors at process exit.
+OpScratch* g_ops_dev[KT_MAX_DEVICES];
 std::mutex g_ops_mu;
 OpScratch& ops_scratch()
 {
     int dev = 0;
     if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= KT_MAX_DEVICES) dev = 0;
-    return g_ops_dev[dev];
+    if (!g_ops_dev[dev]) g_ops_dev[dev] = new OpScratch();
+    return *g_ops_dev[dev];
 }
 #define g_ops (ops_scratch())
 #define KT_OPS_LOCK() std::lock_guard<std::mutex> _ops_lock(g_ops_mu)
 
 int ensure_scratch()
 {
-    if (g_ops.state) return 0;
-    KT_CUDA(cudaMalloc((void**)&g_ops.state, sizeof(OdomState)));
-    KT_CUDA(cudaMemset(g_ops.state, 0, sizeof(OdomState)));
-    KT_CUDA(cudaMalloc((void**)&g_ops.partials, (size_t)MAX_PARTIALS * 32 * sizeof(float)));
-    KT_CUDA(cudaMalloc((void**)&g_ops.ipartials, (size_t)MAX_PARTIALS * 2 * sizeof(int)));
-    KT_CUDA(cudaMalloc((void**)&g_ops.counter, sizeof(unsigned int)));
-    KT_CUDA(cudaMallocHost((void**)&g_ops.host_state, sizeof(OdomState)));
+    if (g_ops.host_state) return 0;
+    Allocations m; const char* W = "operator scratch";
+    OdomState* state; float* partials; int* ipartials; unsigned int* counter; OdomState* host_state;
+    int r;
+    if ((r = m.device(&state, 1, W)) || (r = m.device(&partials, (size_t)MAX_PARTIALS * 32, W)) || (r = m.device(&ipartials, (size_t)MAX_PARTIALS * 2, W)) ||
+        (r = m.device(&counter, 1, W)) || (r = m.pinned(&host_state, 1, W))) return r;
+    KT_CUDA(cudaMemset(state, 0, sizeof(OdomState)));
+    OpScratch& o = g_ops;
+    o.mem = std::move(m); o.state = state; o.partials = partials; o.ipartials = ipartials; o.counter = counter; o.host_state = host_state;
     return 0;
 }
 int ensure_ztable(int vol)
 {
-    if (g_ops.ztable_n >= 2 * vol) return 0;
-    if (g_ops.ztable) cudaFree(g_ops.ztable);
-    KT_CUDA(cudaMalloc((void**)&g_ops.ztable, (size_t)2 * vol * sizeof(float)));
-    g_ops.ztable_n = 2 * vol;
-    return 0;
+    const size_t n = vol > 0 ? (size_t)2 * vol : 0;
+    return g_ops.ztable.grow(n, n, "operator z table");
 }
 
 } // namespace
@@ -139,7 +140,7 @@ int kt_op_integrate(const uint16_t* depth_raw, int rows, int cols, const float* 
     a.Rinv = mat33(Rinv); a.t = make_float3(t[0], t[1], t[2]); a.trunc = trunc; a.tsdf = tsdf; a.color = color; a.vol = vol;
     a.wrap = make_int3(wrap[0], wrap[1], wrap[2]); a.rgb = rgb; a.nmap_curr = nmap_curr; a.angle_color = angle_color != 0;
     a.multi = 0; a.vv = single_volume(tsdf, color, vol);
-    r = integrate(a, g_ops.ztable, st(s)); if (r) return r;
+    r = integrate(a, g_ops.ztable.get(), st(s)); if (r) return r;
     KT_CUDA(cudaStreamSynchronize(st(s)));
     return KT_OK;
 }
@@ -335,20 +336,10 @@ namespace {
 // the operators' small integer scratch, kept between calls so that a call does not allocate
 int place_ints(size_t n, int** out)
 {
-    if (g_ops.place_ints_cap < n) {
-        if (g_ops.place_ints) cudaFree(g_ops.place_ints);
-        g_ops.place_ints = 0; g_ops.place_ints_cap = 0;
-        KT_CUDA(cudaMalloc((void**)&g_ops.place_ints, n * sizeof(int)));
-        g_ops.place_ints_cap = n;
-    }
-    *out = g_ops.place_ints;
+    int r = g_ops.place_ints.grow(n, n, "operator counts"); if (r) return r;
+    *out = g_ops.place_ints.get();
     return 0;
 }
-struct DevBuf {          // scratch of one operator call
-    std::vector<void*> p;
-    template <class T> int get(T** out, size_t n) { void* q = 0; KT_CUDA(cudaMalloc(&q, n ? n * sizeof(T) : 1)); p.push_back(q); *out = (T*)q; return 0; }
-    ~DevBuf() { for (void* q : p) cudaFree(q); }
-};
 }
 
 extern "C" {
@@ -388,8 +379,10 @@ int kt_op_pnp_ransac(const float* p_new, const float* p_old, const float* uv_old
 {
     if (!p_new || !p_old || !uv_old || !k4 || !pose12 || !inliers || !n_inliers || n < 3 || iterations < 1) { set_error("kt_op_pnp_ransac: bad argument"); return KT_ERR_INVALID; }
     KT_OPS_LOCK();
-    DevBuf b; float *pn = 0, *po = 0, *uv = 0; double* pose = 0; unsigned char* in = 0; int* ni = 0; int r;
-    if ((r = b.get(&pn, 3 * (size_t)n)) || (r = b.get(&po, 3 * (size_t)n)) || (r = b.get(&uv, 2 * (size_t)n)) || (r = b.get(&pose, 12)) || (r = b.get(&in, (size_t)n)) || (r = b.get(&ni, 1))) return r;
+    Allocations b; const char* W = "kt_op_pnp_ransac scratch";
+    float *pn, *po, *uv; double* pose; unsigned char* in; int* ni; int r;
+    if ((r = b.device(&pn, 3 * (size_t)n, W)) || (r = b.device(&po, 3 * (size_t)n, W)) || (r = b.device(&uv, 2 * (size_t)n, W)) || (r = b.device(&pose, 12, W)) ||
+        (r = b.device(&in, (size_t)n, W)) || (r = b.device(&ni, 1, W))) return r;
     KT_CUDA(cudaMemcpy(pn, p_new, 12 * (size_t)n, cudaMemcpyHostToDevice));
     KT_CUDA(cudaMemcpy(po, p_old, 12 * (size_t)n, cudaMemcpyHostToDevice));
     KT_CUDA(cudaMemcpy(uv, uv_old, 8 * (size_t)n, cudaMemcpyHostToDevice));
@@ -407,8 +400,9 @@ int kt_op_cloud_fitness(const uint16_t* src_depth, const uint16_t* dst_depth, in
     if (!src_depth || !dst_depth || !k4 || !T12 || !fitness || !n_src || !n_dst || rows <= 0 || cols <= 0) { set_error("kt_op_cloud_fitness: bad argument"); return KT_ERR_INVALID; }
     KT_OPS_LOCK();
     const size_t P = (size_t)rows * cols;
-    DevBuf b; kt_point_xyzrgb *cs = 0, *cd = 0; kt_point_xyzrgbnormal *os = 0, *od = 0; double* d2 = 0; int r;
-    if ((r = b.get(&cs, P)) || (r = b.get(&cd, P)) || (r = b.get(&os, P)) || (r = b.get(&od, P)) || (r = b.get(&d2, P + 8))) return r;
+    Allocations b; const char* W = "kt_op_cloud_fitness scratch";
+    kt_point_xyzrgb *cs, *cd; kt_point_xyzrgbnormal *os, *od; double* d2; int r;
+    if ((r = b.device(&cs, P, W)) || (r = b.device(&cd, P, W)) || (r = b.device(&os, P, W)) || (r = b.device(&od, P, W)) || (r = b.device(&d2, P + 8, W))) return r;
     if ((r = depth_to_cloud(src_depth, rows, cols, intr4(k4), cs, 0)) || (r = depth_to_cloud(dst_depth, rows, cols, intr4(k4), cd, 0))) return r;
     return cloud_fitness(cs, P, cd, P, leaf, T12, &g_ops.slice_ws, &g_ops.fit_ws, os, od, P, d2, fitness, n_src, n_dst, 0);
 }

@@ -392,8 +392,6 @@ deform_apply_kernel(const float4* __restrict__ in, float4* __restrict__ out, con
 
 size_t point_stride(int kind) { return kind == 0 ? sizeof(kt_point_xyzrgbnormal) : kind == 1 ? sizeof(kt_mesh_vertex) : 12; }
 
-template <class T> int dmalloc(T** p, size_t count) { KT_CUDA(cudaMalloc((void**)p, (count ? count : 1) * sizeof(T))); return 0; }
-
 } // namespace
 
 int deform_weights(const float* node_pos, const uint64_t* node_times, int n_nodes, const void* pts, int kind, const uint64_t* times, size_t n,
@@ -462,68 +460,61 @@ int deform_optimise(const float* node_pos, int n, const float* src, const double
     for (int j = 0; j < n; ++j) { x0[12 * j] = 1.0; x0[12 * j + 4] = 1.0; x0[12 * j + 8] = 1.0; }
 
     // ---- device buffers (once per call: the deformation runs once per loop closure) ----
-    int *d_node = 0, *d_off = 0, *d_term = 0, *d_slot = 0; double *d_u = 0, *d_c = 0, *d_rrot = 0, *d_rlin = 0, *d_H = 0, *d_rhs = 0, *d_out = 0;
-    int r = 0;
-    auto cleanup = [&]() { cudaFree(d_node); cudaFree(d_off); cudaFree(d_term); cudaFree(d_slot); cudaFree(d_u); cudaFree(d_c);
-                           cudaFree(d_rrot); cudaFree(d_rlin); cudaFree(d_H); cudaFree(d_rhs); cudaFree(d_out); };
-    auto run = [&]() -> int {
-        const size_t hbytes = (size_t)n * BW * 144 * sizeof(double);
-        if (dmalloc(&d_node, T * DK) || dmalloc(&d_off, n + 1) || dmalloc(&d_term, lterm.size()) || dmalloc(&d_slot, lslot.size()) ||
-            dmalloc(&d_u, tu.size()) || dmalloc(&d_c, tc.size()) || dmalloc(&d_rrot, (size_t)n * 6) || dmalloc(&d_rlin, T * 3) ||
-            dmalloc(&d_H, (size_t)n * BW * 144) || dmalloc(&d_rhs, (size_t)n * 12) || dmalloc(&d_out, 4)) return KT_ERR_CUDA;
-        KT_CUDA(cudaMemcpyAsync(d_node, tnode.data(), tnode.size() * sizeof(int), cudaMemcpyHostToDevice, s));
-        KT_CUDA(cudaMemcpyAsync(d_off, loff.data(), loff.size() * sizeof(int), cudaMemcpyHostToDevice, s));
-        KT_CUDA(cudaMemcpyAsync(d_term, lterm.data(), lterm.size() * sizeof(int), cudaMemcpyHostToDevice, s));
-        KT_CUDA(cudaMemcpyAsync(d_slot, lslot.data(), lslot.size() * sizeof(int), cudaMemcpyHostToDevice, s));
-        KT_CUDA(cudaMemcpyAsync(d_u, tu.data(), tu.size() * sizeof(double), cudaMemcpyHostToDevice, s));
-        KT_CUDA(cudaMemcpyAsync(d_c, tc.data(), tc.size() * sizeof(double), cudaMemcpyHostToDevice, s));
-        KT_CUDA(cudaMemcpyAsync(x_dev, x0.data(), x0.size() * sizeof(double), cudaMemcpyHostToDevice, s));
-        TermsDev td; td.node = d_node; td.u = d_u; td.c = d_c; td.n_terms = (int)T; td.n_con_first = (int)n_reg;
-        td.list_off = d_off; td.list_term = d_term; td.list_slot = d_slot;
-        double out[4];
-        auto residual = [&]() -> int {
-            deform_residual_kernel<<<1, RES_THREADS, 0, s>>>(x_dev, n, td, d_rrot, d_rlin, d_out);
-            KT_LAUNCH_CHECK();
-            return 0;
-        };
-        auto readback = [&]() -> int {
-            KT_CUDA(cudaMemcpyAsync(out, d_out, sizeof(out), cudaMemcpyDeviceToHost, s));
-            KT_CUDA(cudaStreamSynchronize(s));
-            return 0;
-        };
-        // optimiseGraphSparse (:714-774)
-        int rr = residual(); if (rr) return rr;
-        rr = readback(); if (rr) return rr;
-        const float graph_error = (float)(std::sqrt(out[3]) / (double)m);
-        res->constraint_error = graph_error;
-        res->initial_error = res->final_error = out[2];
-        if (graph_error < 0.1) return 0;                                   // "Not deforming, constraint error insignificant"
-        double error = out[2], last = error;
-        int iter = 0;
-        while (iter < 10) {
-            ++iter;
-            KT_CUDA(cudaMemsetAsync(d_H, 0, hbytes, s));
-            deform_assemble_kernel<<<n, ASM_THREADS, 0, s>>>(x_dev, n, td, d_rrot, d_rlin, d_H, d_rhs);
-            KT_LAUNCH_CHECK();
-            deform_solve_kernel<<<1, SOLVE_THREADS, 0, s>>>(d_H, d_rhs, n, x_dev, d_out);
-            KT_LAUNCH_CHECK();
-            rr = residual(); if (rr) return rr;
-            rr = readback(); if (rr) return rr;
-            res->iterations = iter;
-            if (out[1] != 0.0) { res->solver_failed = 1; return 0; }
-            error = out[2];
-            res->final_error = error;
-            const double diff = error - last;
-            if (std::sqrt(out[0]) < 1e-2 || error < 1e-3 || std::fabs(diff) < 1e-5 * error) break;
-            last = error;
-        }
-        res->deformed = 1;
+    Allocations mem(s); const char* W = "deform_optimise scratch";
+    int *d_node, *d_off, *d_term, *d_slot; double *d_u, *d_c, *d_rrot, *d_rlin, *d_H, *d_rhs, *d_out;
+    const size_t hbytes = (size_t)n * BW * 144 * sizeof(double);
+    if (mem.device(&d_node, T * DK, W) || mem.device(&d_off, n + 1, W) || mem.device(&d_term, lterm.size(), W) || mem.device(&d_slot, lslot.size(), W) ||
+        mem.device(&d_u, tu.size(), W) || mem.device(&d_c, tc.size(), W) || mem.device(&d_rrot, (size_t)n * 6, W) || mem.device(&d_rlin, T * 3, W) ||
+        mem.device(&d_H, (size_t)n * BW * 144, W) || mem.device(&d_rhs, (size_t)n * 12, W) || mem.device(&d_out, 4, W)) return KT_ERR_CUDA;
+    KT_CUDA(cudaMemcpyAsync(d_node, tnode.data(), tnode.size() * sizeof(int), cudaMemcpyHostToDevice, s));
+    KT_CUDA(cudaMemcpyAsync(d_off, loff.data(), loff.size() * sizeof(int), cudaMemcpyHostToDevice, s));
+    KT_CUDA(cudaMemcpyAsync(d_term, lterm.data(), lterm.size() * sizeof(int), cudaMemcpyHostToDevice, s));
+    KT_CUDA(cudaMemcpyAsync(d_slot, lslot.data(), lslot.size() * sizeof(int), cudaMemcpyHostToDevice, s));
+    KT_CUDA(cudaMemcpyAsync(d_u, tu.data(), tu.size() * sizeof(double), cudaMemcpyHostToDevice, s));
+    KT_CUDA(cudaMemcpyAsync(d_c, tc.data(), tc.size() * sizeof(double), cudaMemcpyHostToDevice, s));
+    KT_CUDA(cudaMemcpyAsync(x_dev, x0.data(), x0.size() * sizeof(double), cudaMemcpyHostToDevice, s));
+    TermsDev td; td.node = d_node; td.u = d_u; td.c = d_c; td.n_terms = (int)T; td.n_con_first = (int)n_reg;
+    td.list_off = d_off; td.list_term = d_term; td.list_slot = d_slot;
+    double out[4];
+    auto residual = [&]() -> int {
+        deform_residual_kernel<<<1, RES_THREADS, 0, s>>>(x_dev, n, td, d_rrot, d_rlin, d_out);
+        KT_LAUNCH_CHECK();
         return 0;
     };
-    r = run();
-    cleanup();
-    if (r) return r;
-    if (!res->deformed) KT_CUDA(cudaMemcpy(x_dev, x0.data(), x0.size() * sizeof(double), cudaMemcpyHostToDevice));   // undeformed: identity
+    auto readback = [&]() -> int {
+        KT_CUDA(cudaMemcpyAsync(out, d_out, sizeof(out), cudaMemcpyDeviceToHost, s));
+        KT_CUDA(cudaStreamSynchronize(s));
+        return 0;
+    };
+    // optimiseGraphSparse (:714-774)
+    int rr = residual(); if (rr) return rr;
+    rr = readback(); if (rr) return rr;
+    const float graph_error = (float)(std::sqrt(out[3]) / (double)m);
+    res->constraint_error = graph_error;
+    res->initial_error = res->final_error = out[2];
+    // left undeformed: the identity
+    auto identity = [&]() -> int { KT_CUDA(cudaMemcpy(x_dev, x0.data(), x0.size() * sizeof(double), cudaMemcpyHostToDevice)); return 0; };
+    if (graph_error < 0.1) return identity();                          // "Not deforming, constraint error insignificant"
+    double error = out[2], last = error;
+    int iter = 0;
+    while (iter < 10) {
+        ++iter;
+        KT_CUDA(cudaMemsetAsync(d_H, 0, hbytes, s));
+        deform_assemble_kernel<<<n, ASM_THREADS, 0, s>>>(x_dev, n, td, d_rrot, d_rlin, d_H, d_rhs);
+        KT_LAUNCH_CHECK();
+        deform_solve_kernel<<<1, SOLVE_THREADS, 0, s>>>(d_H, d_rhs, n, x_dev, d_out);
+        KT_LAUNCH_CHECK();
+        rr = residual(); if (rr) return rr;
+        rr = readback(); if (rr) return rr;
+        res->iterations = iter;
+        if (out[1] != 0.0) { res->solver_failed = 1; return identity(); }
+        error = out[2];
+        res->final_error = error;
+        const double diff = error - last;
+        if (std::sqrt(out[0]) < 1e-2 || error < 1e-3 || std::fabs(diff) < 1e-5 * error) break;
+        last = error;
+    }
+    res->deformed = 1;
     return 0;
 }
 
@@ -533,7 +524,9 @@ int deform_apply(const float* node_pos, const double* x, int n_nodes, const int3
     if (kind != 0 && kind != 1) { set_error("deform_apply: kind %d", kind); return KT_ERR_INVALID; }
     if (!n) return 0;
     NodeTable* tab = 0;
-    KT_CUDA(cudaMallocAsync((void**)&tab, (size_t)n_nodes * sizeof(NodeTable), s));
+    const size_t bytes = (size_t)n_nodes * sizeof(NodeTable);
+    const cudaError_t e = cudaMallocAsync((void**)&tab, bytes, s);
+    if (e != cudaSuccess) return refused(e, "cudaMallocAsync", "deform_apply node table", bytes);
     deform_node_table_kernel<<<(n_nodes + 127) / 128, 128, 0, s>>>(node_pos, x, n_nodes, tab);
     int r = kt::cuda_check(cudaGetLastError(), "kernel launch", __FILE__, __LINE__); ++g_launches;
     if (!r) {

@@ -1,5 +1,5 @@
 // kintinuous_b200 -- the fused per-frame front end: everything between "a depth / colour frame arrived" and "the odometry can start"
-// in TWO launches (the reference: 12 for ICP-only, 24 + 6 cudaMalloc/cudaFree for the photometric modes).
+// in TWO launches (the reference: 12 for ICP-only, 24 + 6 device allocations / frees for the photometric modes).
 //
 // Replaces (reference, src/frontend/cuda/), as ONE pipeline instead of one kernel + one cudaDeviceSynchronize per function:
 //   launch 1  bilateral_scale_kernel (kt_pyramid.cu)   bilateralFilter (bilateral_pyrdown.cu:60-99) + scaleDepth (tsdf_volume.cu:491-538)

@@ -21,6 +21,7 @@
 #include <dlfcn.h>
 #include <cstdio>
 #include <cstring>
+#include <memory>
 #include <vector>
 
 using namespace kt;
@@ -75,17 +76,23 @@ struct kt_klg {
     FILE* fp; int rows, cols, device; int32_t num_frames; int current; int flip_colors;
     size_t P;
     std::vector<unsigned char> comp_depth, comp_image;       // compressedDepth / compressedImage (RawLogReader.cpp:31-32)
+    Allocations mem;
     uint16_t* depth_pinned[2]; uint8_t* image_pinned[2];      // decompressionBuffer / raw image, pinned
     uint16_t* depth_dev[2]; uint8_t* rgb_dev[2];
     cudaStream_t stream; cudaEvent_t done[2];
     nvjpegHandle_t nvj; nvjpegJpegState_t nvj_state; bool nvj_ready;
     int set;                                                  // buffer set of the frame handed out last
     kt_klg_frame last;
+    ~kt_klg()
+    {
+        cudaSetDevice(device);
+        if (stream) cudaStreamSynchronize(stream);
+        if (nvj_ready) { g_codecs.state_destroy(nvj_state); g_codecs.destroy(nvj); }
+        if (fp) fclose(fp);
+    }
 };
 
 extern "C" {
-
-int kt_klg_close(kt_klg* k);
 
 int kt_klg_open(const char* path, int rows, int cols, int device, kt_klg** out)
 {
@@ -96,40 +103,24 @@ int kt_klg_open(const char* path, int rows, int cols, int device, kt_klg** out)
     if (!fp) { set_error("kt_klg_open: cannot open %s", path); return KT_ERR_INVALID; }
     int32_t n = 0;
     if (fread(&n, sizeof(int32_t), 1, fp) != 1 || n < 0) { fclose(fp); set_error("kt_klg_open: %s has no frame count", path); return KT_ERR_INVALID; }
-    kt_klg* k = new kt_klg();
+    std::unique_ptr<kt_klg> k(new kt_klg());
     k->fp = fp; k->rows = rows; k->cols = cols; k->device = device; k->num_frames = n; k->current = 0; k->flip_colors = 0; k->set = 1;
     k->P = (size_t)rows * cols;
     k->comp_depth.resize(k->P * 2); k->comp_image.resize(k->P * 3);
-    cudaError_t e = cudaSuccess;
-    for (int i = 0; i < 2 && e == cudaSuccess; ++i) {
-        if ((e = cudaMallocHost((void**)&k->depth_pinned[i], k->P * 2)) != cudaSuccess) break;
-        if ((e = cudaMallocHost((void**)&k->image_pinned[i], k->P * 3)) != cudaSuccess) break;
-        if ((e = cudaMalloc((void**)&k->depth_dev[i], k->P * 2)) != cudaSuccess) break;
-        if ((e = cudaMalloc((void**)&k->rgb_dev[i], k->P * 3)) != cudaSuccess) break;
-        if ((e = cudaEventCreateWithFlags(&k->done[i], cudaEventDisableTiming)) != cudaSuccess) break;
-    }
-    if (e == cudaSuccess) e = cudaStreamCreateWithFlags(&k->stream, cudaStreamNonBlocking);
-    if (e != cudaSuccess) { kt_klg_close(k); return cuda_check(e, "kt_klg_open: buffers", __FILE__, __LINE__); }
+    const char* W = "kt_klg_open buffers";
+    int r;
+    for (int i = 0; i < 2; ++i)
+        if ((r = k->mem.pinned(&k->depth_pinned[i], k->P, W)) || (r = k->mem.pinned(&k->image_pinned[i], k->P * 3, W)) ||
+            (r = k->mem.device(&k->depth_dev[i], k->P, W)) || (r = k->mem.device(&k->rgb_dev[i], k->P * 3, W)) ||
+            (r = k->mem.event(&k->done[i], cudaEventDisableTiming, W))) return r;
+    if ((r = k->mem.stream(&k->stream, W))) return r;
     memset(&k->last, 0, sizeof(k->last));
-    *out = k;
+    *out = k.release();
     return KT_OK;
 }
 
 int kt_klg_close(kt_klg* k)
 {
-    if (!k) return KT_OK;
-    cudaSetDevice(k->device);
-    if (k->stream) cudaStreamSynchronize(k->stream);
-    if (k->nvj_ready) { g_codecs.state_destroy(k->nvj_state); g_codecs.destroy(k->nvj); }
-    for (int i = 0; i < 2; ++i) {
-        if (k->depth_pinned[i]) cudaFreeHost(k->depth_pinned[i]);
-        if (k->image_pinned[i]) cudaFreeHost(k->image_pinned[i]);
-        if (k->depth_dev[i]) cudaFree(k->depth_dev[i]);
-        if (k->rgb_dev[i]) cudaFree(k->rgb_dev[i]);
-        if (k->done[i]) cudaEventDestroy(k->done[i]);
-    }
-    if (k->stream) cudaStreamDestroy(k->stream);
-    if (k->fp) fclose(k->fp);
     delete k;
     return KT_OK;
 }

@@ -172,17 +172,6 @@ map_rigid_kernel(kt_point_xyzrgbnormal* __restrict__ p, size_t n, const RigidF C
 
 int grid_for(size_t n) { const size_t b = (n + MAP_THREADS - 1) / MAP_THREADS, cap = (size_t)device_info().sm_count * 16; return (int)(b < 1 ? 1 : (b > cap ? cap : b)); }
 
-// cudaMalloc that leaves no sticky "last error" behind on failure (a later launch check would report it)
-int map_alloc(void** p, size_t bytes, const char* who)
-{
-    if (cudaMalloc(p, bytes ? bytes : 1) != cudaSuccess) {
-        cudaGetLastError(); *p = 0;
-        set_error("%s: cannot allocate %zu bytes of device memory", who, bytes);
-        return KT_ERR_CUDA;
-    }
-    return 0;
-}
-
 // Stage timing of one voxel_grid call (CUDA events on its stream)
 struct MapEvents {
     cudaEvent_t e[4]; bool on;
@@ -202,90 +191,84 @@ int voxel_grid_impl(const unsigned char* in, size_t n, float leaf, unsigned char
                     float* ms2, cudaStream_t s)
 {
     const char* who = "voxel_grid";
-    unsigned int* bounds = 0; void* ws = 0; void* tmp = 0;
-    auto cleanup = [&]() { cudaStreamSynchronize(s); cudaFree(bounds); cudaFree(ws); cudaFree(tmp); };
     MapEvents ev(ms2 != 0);
-    auto run = [&]() -> int {
-        unsigned int host[7] = {0xffffffffu, 0xffffffffu, 0xffffffffu, 0u, 0u, 0u, 0u};
-        int r = map_alloc((void**)&bounds, sizeof(host), who); if (r) return r;
-        KT_CUDA(cudaMemcpyAsync(bounds, host, sizeof(host), cudaMemcpyHostToDevice, s));
-        map_bounds_kernel<REC><<<grid_for(n), MAP_THREADS, 0, s>>>(in, n, bounds);
-        KT_LAUNCH_CHECK();
-        KT_CUDA(cudaMemcpyAsync(host, bounds, sizeof(host), cudaMemcpyDeviceToHost, s));
-        KT_CUDA(cudaStreamSynchronize(s));
-        if (host[6]) { set_error("%s: %u points have a non-finite x, y or z", who, host[6]); return KT_ERR_INVALID; }
-        float mn[3], mx[3];
-        for (int a = 0; a < 3; ++a) { mn[a] = unord_f(host[a]); mx[a] = unord_f(host[3 + a]); }
-        MapGrid g; g.inv = 1.0f / leaf;                                   // inverse_leaf_size_ = 1 / leaf_size_ (float)
-        long long min_b[3], div_b[3], top[3];
-        for (int a = 0; a < 3; ++a) {
-            const float lo = std::floor(mn[a] * g.inv), hi = std::floor(mx[a] * g.inv);
-            if (!(lo >= -2147483648.0f && hi < 2147483648.0f)) {
-                set_error("%s: the leaf grid's bounds (%g .. %g leaves on axis %d) do not fit an int", who, (double)lo, (double)hi, a); return KT_ERR_INVALID; }
-            min_b[a] = (long long)lo; div_b[a] = (long long)hi - min_b[a] + 1;
-            g.min_b[a] = lo;
-            // largest leaf coordinate: floor(p * inv) - (float)min_b is a float difference, exact below 2^24, rounded above
-            top[a] = (long long)(float)(div_b[a] - 1);
-        }
-        // largest key, checked against 2^62 (every product below stays under 2^64: each factor < 2^33, checked step by step)
-        const unsigned long long LIM = 1ull << 62;
-        const unsigned long long d0 = (unsigned long long)div_b[0], d1 = (unsigned long long)div_b[1];
-        if (d1 > LIM / d0) { set_error("%s: the leaf grid has more than 2^62 cells", who); return KT_ERR_INVALID; }
-        g.mul1 = d0; g.mul2 = d0 * d1;
-        if ((unsigned long long)top[2] > LIM / g.mul2) { set_error("%s: the leaf grid has more than 2^62 cells", who); return KT_ERR_INVALID; }
-        const unsigned long long kmax = (unsigned long long)top[0] + (unsigned long long)top[1] * g.mul1 + (unsigned long long)top[2] * g.mul2;
-        if (kmax > LIM) { set_error("%s: the leaf grid has more than 2^62 cells", who); return KT_ERR_INVALID; }
-        // voxel_grid.hpp's overflow check, in int64 as PCL computes it: PCL would return the cloud unfiltered
-        const long long dx = (long long)((mx[0] - mn[0]) * g.inv) + 1, dy = (long long)((mx[1] - mn[1]) * g.inv) + 1, dz = (long long)((mx[2] - mn[2]) * g.inv) + 1;
-        *pcl_would_skip = (__int128)dx * dy * dz > (__int128)2147483647 ? 1 : 0;
-        int bits = 1;
-        while (bits < 64 && (kmax >> bits) != 0) ++bits;
+    Allocations mem(s);
+    unsigned int host[7] = {0xffffffffu, 0xffffffffu, 0xffffffffu, 0u, 0u, 0u, 0u};
+    unsigned int* bounds = 0; unsigned char* w = 0; unsigned char* tmp = 0;
+    int r = mem.device(&bounds, 7, "voxel_grid bounds"); if (r) return r;
+    KT_CUDA(cudaMemcpyAsync(bounds, host, sizeof(host), cudaMemcpyHostToDevice, s));
+    map_bounds_kernel<REC><<<grid_for(n), MAP_THREADS, 0, s>>>(in, n, bounds);
+    KT_LAUNCH_CHECK();
+    KT_CUDA(cudaMemcpyAsync(host, bounds, sizeof(host), cudaMemcpyDeviceToHost, s));
+    KT_CUDA(cudaStreamSynchronize(s));
+    if (host[6]) { set_error("%s: %u points have a non-finite x, y or z", who, host[6]); return KT_ERR_INVALID; }
+    float mn[3], mx[3];
+    for (int a = 0; a < 3; ++a) { mn[a] = unord_f(host[a]); mx[a] = unord_f(host[3 + a]); }
+    MapGrid g; g.inv = 1.0f / leaf;                                   // inverse_leaf_size_ = 1 / leaf_size_ (float)
+    long long min_b[3], div_b[3], top[3];
+    for (int a = 0; a < 3; ++a) {
+        const float lo = std::floor(mn[a] * g.inv), hi = std::floor(mx[a] * g.inv);
+        if (!(lo >= -2147483648.0f && hi < 2147483648.0f)) {
+            set_error("%s: the leaf grid's bounds (%g .. %g leaves on axis %d) do not fit an int", who, (double)lo, (double)hi, a); return KT_ERR_INVALID; }
+        min_b[a] = (long long)lo; div_b[a] = (long long)hi - min_b[a] + 1;
+        g.min_b[a] = lo;
+        // largest leaf coordinate: floor(p * inv) - (float)min_b is a float difference, exact below 2^24, rounded above
+        top[a] = (long long)(float)(div_b[a] - 1);
+    }
+    // largest key, checked against 2^62 (every product below stays under 2^64: each factor < 2^33, checked step by step)
+    const unsigned long long LIM = 1ull << 62;
+    const unsigned long long d0 = (unsigned long long)div_b[0], d1 = (unsigned long long)div_b[1];
+    if (d1 > LIM / d0) { set_error("%s: the leaf grid has more than 2^62 cells", who); return KT_ERR_INVALID; }
+    g.mul1 = d0; g.mul2 = d0 * d1;
+    if ((unsigned long long)top[2] > LIM / g.mul2) { set_error("%s: the leaf grid has more than 2^62 cells", who); return KT_ERR_INVALID; }
+    const unsigned long long kmax = (unsigned long long)top[0] + (unsigned long long)top[1] * g.mul1 + (unsigned long long)top[2] * g.mul2;
+    if (kmax > LIM) { set_error("%s: the leaf grid has more than 2^62 cells", who); return KT_ERR_INVALID; }
+    // voxel_grid.hpp's overflow check, in int64 as PCL computes it: PCL would return the cloud unfiltered
+    const long long dx = (long long)((mx[0] - mn[0]) * g.inv) + 1, dy = (long long)((mx[1] - mn[1]) * g.inv) + 1, dz = (long long)((mx[2] - mn[2]) * g.inv) + 1;
+    *pcl_would_skip = (__int128)dx * dy * dz > (__int128)2147483647 ? 1 : 0;
+    int bits = 1;
+    while (bits < 64 && (kmax >> bits) != 0) ++bits;
 
-        // workspace: keys x 2, indices x 2, head flags, scan, starts (n + 1), leaf count
-        const unsigned int nn = (unsigned int)n;
-        const size_t off_k1 = (size_t)n * 8, off_i0 = off_k1 + (size_t)n * 8, off_i1 = off_i0 + (size_t)n * 4, off_h = off_i1 + (size_t)n * 4,
-                     off_s = off_h + (size_t)n * 4, off_st = off_s + (size_t)n * 4, off_m = off_st + ((size_t)n + 1) * 4, total = off_m + 16;
-        if ((r = map_alloc(&ws, total, who))) return r;
-        unsigned char* w = (unsigned char*)ws;
-        unsigned long long* k0 = (unsigned long long*)w; unsigned long long* k1 = (unsigned long long*)(w + off_k1);
-        unsigned int* i0 = (unsigned int*)(w + off_i0); unsigned int* i1 = (unsigned int*)(w + off_i1);
-        unsigned int* head = (unsigned int*)(w + off_h); unsigned int* slot = (unsigned int*)(w + off_s);
-        unsigned int* starts = (unsigned int*)(w + off_st); unsigned int* n_leaves = (unsigned int*)(w + off_m);
-        cub::DoubleBuffer<unsigned long long> kb(k0, k1); cub::DoubleBuffer<unsigned int> vb(i0, i1);
-        size_t sort_bytes = 0, scan_bytes = 0;
-        KT_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, sort_bytes, kb, vb, nn, 0, bits, s));
-        KT_CUDA(cub::DeviceScan::ExclusiveSum(nullptr, scan_bytes, head, slot, nn, s));
-        if ((r = map_alloc(&tmp, std::max(sort_bytes, scan_bytes), who))) return r;
+    // workspace: keys x 2, indices x 2, head flags, scan, starts (n + 1), leaf count
+    const unsigned int nn = (unsigned int)n;
+    const size_t off_k1 = (size_t)n * 8, off_i0 = off_k1 + (size_t)n * 8, off_i1 = off_i0 + (size_t)n * 4, off_h = off_i1 + (size_t)n * 4,
+                 off_s = off_h + (size_t)n * 4, off_st = off_s + (size_t)n * 4, off_m = off_st + ((size_t)n + 1) * 4, total = off_m + 16;
+    if ((r = mem.device(&w, total, "voxel_grid keys and indices"))) return r;
+    unsigned long long* k0 = (unsigned long long*)w; unsigned long long* k1 = (unsigned long long*)(w + off_k1);
+    unsigned int* i0 = (unsigned int*)(w + off_i0); unsigned int* i1 = (unsigned int*)(w + off_i1);
+    unsigned int* head = (unsigned int*)(w + off_h); unsigned int* slot = (unsigned int*)(w + off_s);
+    unsigned int* starts = (unsigned int*)(w + off_st); unsigned int* n_leaves = (unsigned int*)(w + off_m);
+    cub::DoubleBuffer<unsigned long long> kb(k0, k1); cub::DoubleBuffer<unsigned int> vb(i0, i1);
+    size_t sort_bytes = 0, scan_bytes = 0;
+    KT_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, sort_bytes, kb, vb, nn, 0, bits, s));
+    KT_CUDA(cub::DeviceScan::ExclusiveSum(nullptr, scan_bytes, head, slot, nn, s));
+    if ((r = mem.device(&tmp, std::max(sort_bytes, scan_bytes), "voxel_grid sort storage"))) return r;
 
-        ev.mark(0, s);
-        map_keys_kernel<REC><<<grid_for(n), MAP_THREADS, 0, s>>>(in, n, g, k0, i0);
+    ev.mark(0, s);
+    map_keys_kernel<REC><<<grid_for(n), MAP_THREADS, 0, s>>>(in, n, g, k0, i0);
+    KT_LAUNCH_CHECK();
+    KT_CUDA(cub::DeviceRadixSort::SortPairs(tmp, sort_bytes, kb, vb, nn, 0, bits, s));
+    ev.mark(1, s);
+    const unsigned long long* keys = kb.Current(); const unsigned int* idx = vb.Current();
+    const int blocks = (int)((n + MAP_THREADS - 1) / MAP_THREADS);
+    map_heads_kernel<<<blocks, MAP_THREADS, 0, s>>>(keys, nn, head);
+    KT_LAUNCH_CHECK();
+    KT_CUDA(cub::DeviceScan::ExclusiveSum(tmp, scan_bytes, head, slot, nn, s));
+    map_starts_kernel<<<blocks, MAP_THREADS, 0, s>>>(head, slot, nn, starts, n_leaves);
+    KT_LAUNCH_CHECK();
+    unsigned int m = 0;
+    KT_CUDA(cudaMemcpyAsync(&m, n_leaves, sizeof(m), cudaMemcpyDeviceToHost, s));
+    KT_CUDA(cudaStreamSynchronize(s));
+    const unsigned int n_out = (unsigned int)std::min((size_t)m, capacity);
+    if (out && n_out) {
+        map_centroid_kernel<REC><<<div_up((int)n_out, MAP_THREADS), MAP_THREADS, 0, s>>>(in, idx, starts, n_out, out);
         KT_LAUNCH_CHECK();
-        KT_CUDA(cub::DeviceRadixSort::SortPairs(tmp, sort_bytes, kb, vb, nn, 0, bits, s));
-        ev.mark(1, s);
-        const unsigned long long* keys = kb.Current(); const unsigned int* idx = vb.Current();
-        const int blocks = (int)((n + MAP_THREADS - 1) / MAP_THREADS);
-        map_heads_kernel<<<blocks, MAP_THREADS, 0, s>>>(keys, nn, head);
-        KT_LAUNCH_CHECK();
-        KT_CUDA(cub::DeviceScan::ExclusiveSum(tmp, scan_bytes, head, slot, nn, s));
-        map_starts_kernel<<<blocks, MAP_THREADS, 0, s>>>(head, slot, nn, starts, n_leaves);
-        KT_LAUNCH_CHECK();
-        unsigned int m = 0;
-        KT_CUDA(cudaMemcpyAsync(&m, n_leaves, sizeof(m), cudaMemcpyDeviceToHost, s));
-        KT_CUDA(cudaStreamSynchronize(s));
-        const unsigned int n_out = (unsigned int)std::min((size_t)m, capacity);
-        if (out && n_out) {
-            map_centroid_kernel<REC><<<div_up((int)n_out, MAP_THREADS), MAP_THREADS, 0, s>>>(in, idx, starts, n_out, out);
-            KT_LAUNCH_CHECK();
-        }
-        ev.mark(2, s);
-        KT_CUDA(cudaStreamSynchronize(s));
-        if (ms2) { ms2[0] = ev.ms(0, 1); ms2[1] = ev.ms(1, 2); }
-        *count = m;
-        return 0;
-    };
-    const int r = run();
-    cleanup();
-    return r;
+    }
+    ev.mark(2, s);
+    KT_CUDA(cudaStreamSynchronize(s));
+    if (ms2) { ms2[0] = ev.ms(0, 1); ms2[1] = ev.ms(1, 2); }
+    *count = m;
+    return 0;
 }
 
 } // namespace

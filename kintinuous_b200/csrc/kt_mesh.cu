@@ -254,16 +254,7 @@ MeshParams make_params(const MeshArgs& a)
     return p;
 }
 
-template <class T> int grow(T** ptr, size_t* cap, size_t n)
-{
-    if (n <= *cap) return 0;
-    if (*ptr) cudaFree(*ptr);
-    *ptr = 0; *cap = 0;
-    const size_t want = n + n / 4 + 256;
-    KT_CUDA(cudaMalloc((void**)ptr, want * sizeof(T)));
-    *cap = want;
-    return 0;
-}
+size_t with_slack(size_t n) { return n + n / 4 + 256; }      // capacity of a grown workspace buffer
 
 } // namespace
 
@@ -274,19 +265,20 @@ int mesh_count(const MeshArgs& a, MeshWorkspace* ws, size_t* n_verts, size_t* n_
     if (p.total == 0) return 0;
     const long long nb = (p.total + MESH_TILE - 1) / MESH_TILE;
     if (nb > 0x7fffffffLL) { set_error("mesh: box too large"); return KT_ERR_INVALID; }
-    int r = grow(&ws->counts, &ws->counts_cap, (size_t)4 * (nb + 1)); if (r) return r;
-    if (!ws->totals_host) KT_CUDA(cudaMallocHost((void**)&ws->totals_host, 2 * sizeof(unsigned long long)));
-    unsigned long long* vc = ws->counts; unsigned long long* tc = vc + (nb + 1);
+    const size_t n = (size_t)4 * (nb + 1);
+    int r = ws->counts.grow(n, with_slack(n), "mesh tile counts"); if (r) return r;
+    if (!ws->totals_host && (r = ws->fixed.pinned(&ws->totals_host, 2, "mesh totals"))) return r;
+    unsigned long long* vc = ws->counts.get(); unsigned long long* tc = vc + (nb + 1);
     unsigned long long* vo = tc + (nb + 1); unsigned long long* to = vo + (nb + 1);
     mesh_count_kernel<<<(unsigned int)nb, MESH_THREADS, 0, s>>>(p, vc, tc);
     KT_LAUNCH_CHECK();
     size_t need = 0;
     KT_CUDA(cub::DeviceScan::ExclusiveSum(nullptr, need, vc, vo, (int)(nb + 1), s));
-    r = grow((unsigned char**)&ws->tmp, &ws->tmp_cap, need); if (r) return r;
-    size_t have = ws->tmp_cap;
-    KT_CUDA(cub::DeviceScan::ExclusiveSum(ws->tmp, have, vc, vo, (int)(nb + 1), s));
-    have = ws->tmp_cap;
-    KT_CUDA(cub::DeviceScan::ExclusiveSum(ws->tmp, have, tc, to, (int)(nb + 1), s));
+    r = ws->tmp.grow(need, with_slack(need), "mesh scan storage"); if (r) return r;
+    size_t have = ws->tmp.capacity();
+    KT_CUDA(cub::DeviceScan::ExclusiveSum(ws->tmp.get(), have, vc, vo, (int)(nb + 1), s));
+    have = ws->tmp.capacity();
+    KT_CUDA(cub::DeviceScan::ExclusiveSum(ws->tmp.get(), have, tc, to, (int)(nb + 1), s));
     KT_CUDA(cudaMemcpyAsync(&ws->totals_host[0], vo + nb, sizeof(unsigned long long), cudaMemcpyDeviceToHost, s));
     KT_CUDA(cudaMemcpyAsync(&ws->totals_host[1], to + nb, sizeof(unsigned long long), cudaMemcpyDeviceToHost, s));
     KT_CUDA(cudaStreamSynchronize(s));
@@ -300,22 +292,13 @@ int mesh_emit(const MeshArgs& a, MeshWorkspace* ws, size_t n_verts, void* verts,
     if (p.total == 0 || n_verts == 0) return 0;
     if (n_verts > 0xffffffffull) { set_error("mesh: %zu vertices do not fit 32-bit indices", n_verts); return KT_ERR_CAPACITY; }
     const long long nb = (p.total + MESH_TILE - 1) / MESH_TILE;
-    int r = grow(&ws->keys, &ws->keys_cap, n_verts); if (r) return r;
-    const unsigned long long* vo = ws->counts + 2 * (nb + 1); const unsigned long long* to = vo + (nb + 1);
-    mesh_vertex_kernel<<<(unsigned int)nb, MESH_THREADS, 0, s>>>(p, vo, (uint4*)verts, ws->keys);
+    int r = ws->keys.grow(n_verts, with_slack(n_verts), "mesh vertex keys"); if (r) return r;
+    const unsigned long long* vo = ws->counts.get() + 2 * (nb + 1); const unsigned long long* to = vo + (nb + 1);
+    mesh_vertex_kernel<<<(unsigned int)nb, MESH_THREADS, 0, s>>>(p, vo, (uint4*)verts, ws->keys.get());
     KT_LAUNCH_CHECK();
-    mesh_triangle_kernel<<<(unsigned int)nb, MESH_THREADS, 0, s>>>(p, to, ws->keys, n_verts, tris);
+    mesh_triangle_kernel<<<(unsigned int)nb, MESH_THREADS, 0, s>>>(p, to, ws->keys.get(), n_verts, tris);
     KT_LAUNCH_CHECK();
     return 0;
-}
-
-void mesh_ws_free(MeshWorkspace* ws)
-{
-    if (ws->counts) cudaFree(ws->counts);
-    if (ws->tmp) cudaFree(ws->tmp);
-    if (ws->keys) cudaFree(ws->keys);
-    if (ws->totals_host) cudaFreeHost(ws->totals_host);
-    *ws = MeshWorkspace();
 }
 
 } // namespace kt

@@ -2,6 +2,7 @@
 // the tracker in kt_tracker.cu call these).  All pointers are device pointers, compact pitch.
 #pragma once
 #include "kt_common.cuh"
+#include "kt_mem.hpp"
 
 struct kt_deform_report;
 struct kt_pgo_report;
@@ -164,27 +165,28 @@ int extract_slice_mg(const VolumeView& vv, const float3& volume_size, int vol, v
                      int minX, int maxX, int minY, int maxY, int minZ, int maxZ, int subsample,
                      const int3& real_wrap, unsigned int* counter_dev, cudaStream_t s);
 // ---- slice post-processing (kt_slice.cu): CloudSliceProcessor.cpp:97-162 on the device ----
-struct SliceWorkspace { unsigned int* mask; unsigned int* word_off; unsigned int* block_tot; size_t words_cap; void* acc; size_t acc_cap; unsigned int* bounds; unsigned int* bounds_host; };
+struct SliceWorkspace {
+    DeviceBuffer<unsigned int> mask, word_off, block_tot;    // leaf bitmap, its word offsets and scan block totals (grown together)
+    DeviceBuffer<unsigned char> acc;                         // per-leaf accumulators
+    Allocations fixed; unsigned int* bounds = nullptr; unsigned int* bounds_host = nullptr;
+};
 int process_slice(const void* points_dev /* kt_point_xyzrgb */, size_t n, int weight_cull, float leaf, int k_search, void* out_dev /* kt_point_xyzrgbnormal */,
                   size_t capacity, size_t* count, SliceWorkspace* ws, cudaStream_t s);
-void slice_ws_free(SliceWorkspace* ws);
 // ---- marching cubes over a box of the cyclic volume (kt_mesh.cu): an indexed mesh in a fixed order, see the file header ----
 struct MeshArgs {
     const int16_t* tsdf; const uint8_t* color; int vol; float3 volume_size; int3 wrap; int3 real_wrap;   // wrap / real_wrap: as extract_slice
     int minX, maxX, minY, maxY, minZ, maxZ; int weight_cull;
 };
 struct MeshWorkspace {
-    unsigned long long* counts; size_t counts_cap;    // per-tile vertex / triangle totals and their exclusive scans
-    void* tmp; size_t tmp_cap;                        // CUB scan storage
-    unsigned long long* keys; size_t keys_cap;        // 3 * owner + axis of every vertex, ascending
-    unsigned long long* totals_host;                  // pinned: vertex and triangle counts
-    MeshWorkspace() : counts(0), counts_cap(0), tmp(0), tmp_cap(0), keys(0), keys_cap(0), totals_host(0) {}
+    DeviceBuffer<unsigned long long> counts;          // per-tile vertex / triangle totals and their exclusive scans
+    DeviceBuffer<unsigned char> tmp;                  // CUB scan storage
+    DeviceBuffer<unsigned long long> keys;            // 3 * owner + axis of every vertex, ascending
+    Allocations fixed; unsigned long long* totals_host = nullptr;      // pinned: vertex and triangle counts
 };
 // count + scan, then one read-back (synchronises s): the mesh's vertex and triangle counts
 int mesh_count(const MeshArgs& a, MeshWorkspace* ws, size_t* n_verts, size_t* n_tris, cudaStream_t s);
 // after mesh_count with the same arguments: writes n_verts 32-byte kt_mesh_vertex records and the triangles (3 x uint32 each); asynchronous
 int mesh_emit(const MeshArgs& a, MeshWorkspace* ws, size_t n_verts, void* verts, uint32_t* tris, cudaStream_t s);
-void mesh_ws_free(MeshWorkspace* ws);
 // ---- embedded deformation graph (kt_deform.cu, host logic in kt_deform.hpp) ----
 // Node positions: float n x 3 (device), node times ascending.  kind: 0 kt_point_xyzrgbnormal, 1 kt_mesh_vertex, 2 packed float xyz.
 // Writes 4 node ids (int32, ascending) and 4 FP64 weights per point; asynchronous.
@@ -204,12 +206,12 @@ struct PgoFactor;
 // Synchronises s.
 int pgo_optimise(const double* poses_in, int n, const PgoFactor* factors, int n_factors, double* X, kt_pgo_report* rep, cudaStream_t s);
 // ---- place recognition (kt_surf.cu, kt_place.cu, cloud_fitness in kt_slice.cu; host logic in kt_place.hpp) ----
-struct SurfWorkspace {
-    int rows, cols; int* integral; float* resp; void* cand; unsigned long long* keys; unsigned int* idx; unsigned int* n_cand; void* tmp; size_t tmp_bytes;
-    SurfWorkspace() : rows(0), cols(0), integral(0), resp(0), cand(0), keys(0), idx(0), n_cand(0), tmp(0), tmp_bytes(0) {}
+struct SurfWorkspace {          // sized for one image shape
+    int rows = 0, cols = 0; Allocations mem;
+    int* integral = nullptr; float* resp = nullptr; void* cand = nullptr; unsigned long long* keys = nullptr; unsigned int* idx = nullptr;
+    unsigned int* n_cand = nullptr; unsigned char* tmp = nullptr; size_t tmp_bytes = 0;
 };
 int surf_ws_reserve(SurfWorkspace* ws, int rows, int cols);
-void surf_ws_free(SurfWorkspace* ws);
 // RGB image -> at most max_features keypoints, strongest first: kp 6 floats each (x, y, size, angle in radians, response, laplacian sign),
 // desc 64 floats each, *n_out_dev (device) = keypoints written.  Asynchronous.
 int surf(const uint8_t* rgb, int rows, int cols, float threshold, int max_features, float* kp, float* desc, int* n_out_dev, SurfWorkspace* ws, cudaStream_t s);
@@ -220,10 +222,9 @@ int keypoints_3d(const float* kp, const int* n_dev, int max_n, const uint16_t* d
 int match_ratio(const float* db, int n_seg, int stride, const int* seg_count_dev, const float* q, const int* n_query_dev, int q_cap, float ratio,
                 int* best, float* d1, float* d2, unsigned char* pass, int* seg_passes, cudaStream_t s);
 struct PnpArgs { const float* p_new; const float* p_old; const float* uv_old; int n; Intr k; int iterations; float threshold_px; unsigned long long seed; };
-struct PnpWorkspace { int* counts; double* hyps; unsigned int* counter; int cap; PnpWorkspace() : counts(0), hyps(0), counter(0), cap(0) {} };
+struct PnpWorkspace { DeviceBuffer<int> counts; DeviceBuffer<double> hyps; DeviceBuffer<unsigned int> counter; };
 // pose12 (device, FP64): R row-major + t with R p_new + t in the old camera; inliers (device) per match; *n_inliers (device)
 int pnp_ransac(const PnpArgs& a, PnpWorkspace* ws, double* pose12, unsigned char* inliers, int* n_inliers, cudaStream_t s);
-void pnp_ws_free(PnpWorkspace* ws);
 // depth (u16 mm) -> rows*cols kt_point_xyzrgb, alpha 1 where the depth is valid
 int depth_to_cloud(const uint16_t* depth, int rows, int cols, const Intr& k, void* cloud, cudaStream_t s);
 // getFitnessScore of the loop check: d2_dev holds capacity + 8 doubles; synchronises s

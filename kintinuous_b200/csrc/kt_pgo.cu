@@ -480,14 +480,6 @@ __global__ void pgo_update_kernel(int n, const double* __restrict__ dx, double* 
     for (int r = 0; r < 3; ++r) { for (int c = 0; c < 3; ++c) P[4 * r + c] = R[3 * r + c]; P[4 * r + 3] += d[r]; }
 }
 
-template <class T> int dalloc(std::vector<void*>& owned, T** p, size_t count)
-{
-    void* q = 0;
-    KT_CUDA(cudaMalloc(&q, (count ? count : 1) * sizeof(T)));
-    owned.push_back(q); *p = (T*)q;
-    return 0;
-}
-
 } // namespace
 
 int pgo_optimise(const double* poses_in, int n, const PgoFactor* fh, int nf, double* X, kt_pgo_report* rep, cudaStream_t s)
@@ -505,94 +497,88 @@ int pgo_optimise(const double* poses_in, int n, const PgoFactor* fh, int nf, dou
     const int top = plan.top(), K = plan.n[top], N = 6 * K;
     std::vector<int> loff, lidx; pgo_loop_csr(fh, nf, n, loff, lidx);
 
-    std::vector<void*> owned;
-    cudaEvent_t ev[2] = {0, 0};
-    auto run = [&]() -> int {
-        PgoFactor* d_f; double *d_E, *d_JI, *d_JJ, *d_e2, *d_HL, *d_out, *d_M, *d_Lf; int *d_loff, *d_lidx, *d_fail, *d_ti, *d_tj;
-        if (dalloc(owned, &d_f, nf) || dalloc(owned, &d_E, 6 * (size_t)nf) || dalloc(owned, &d_JI, 36 * (size_t)nf) || dalloc(owned, &d_JJ, 36 * (size_t)nf) ||
-            dalloc(owned, &d_e2, nf) || dalloc(owned, &d_HL, 36 * (size_t)(L ? L : 1)) || dalloc(owned, &d_out, 2) || dalloc(owned, &d_M, (size_t)N * N) ||
-            dalloc(owned, &d_Lf, (size_t)N * N) || dalloc(owned, &d_loff, n + 1) || dalloc(owned, &d_lidx, lidx.size()) || dalloc(owned, &d_fail, 1) ||
-            dalloc(owned, &d_ti, L) || dalloc(owned, &d_tj, L)) return KT_ERR_CUDA;
-        // per level: D, C, g, A, x; per level below the top: sep and the segment outputs
-        std::vector<double*> D(top + 1), C(top + 1), g(top + 1), A(top + 1), x(top + 1);
-        std::vector<int*> sep(top);
-        std::vector<double*> Saa(top), Sbb(top), Sba(top), ga(top), gb(top);
-        for (int l = 0; l <= top; ++l) {
-            const size_t m = plan.n[l];
-            if (dalloc(owned, &D[l], 36 * m) || dalloc(owned, &C[l], 36 * m) || dalloc(owned, &g[l], 6 * m) || dalloc(owned, &A[l], 36 * m) || dalloc(owned, &x[l], 6 * m)) return KT_ERR_CUDA;
-            if (l < top) {
-                const size_t S = plan.sep[l].size() - 1;
-                if (dalloc(owned, &sep[l], S + 1) || dalloc(owned, &Saa[l], 36 * S) || dalloc(owned, &Sbb[l], 36 * S) || dalloc(owned, &Sba[l], 36 * S) ||
-                    dalloc(owned, &ga[l], 6 * S) || dalloc(owned, &gb[l], 6 * S)) return KT_ERR_CUDA;
-                KT_CUDA(cudaMemcpyAsync(sep[l], plan.sep[l].data(), (S + 1) * sizeof(int), cudaMemcpyHostToDevice, s));
-            }
+    Allocations mem(s); const char* W = "pgo_optimise scratch";
+    PgoFactor* d_f; double *d_E, *d_JI, *d_JJ, *d_e2, *d_HL, *d_out, *d_M, *d_Lf; int *d_loff, *d_lidx, *d_fail, *d_ti, *d_tj;
+    if (mem.device(&d_f, nf, W) || mem.device(&d_E, 6 * (size_t)nf, W) || mem.device(&d_JI, 36 * (size_t)nf, W) || mem.device(&d_JJ, 36 * (size_t)nf, W) ||
+        mem.device(&d_e2, nf, W) || mem.device(&d_HL, 36 * (size_t)(L ? L : 1), W) || mem.device(&d_out, 2, W) || mem.device(&d_M, (size_t)N * N, W) ||
+        mem.device(&d_Lf, (size_t)N * N, W) || mem.device(&d_loff, n + 1, W) || mem.device(&d_lidx, lidx.size(), W) || mem.device(&d_fail, 1, W) ||
+        mem.device(&d_ti, L, W) || mem.device(&d_tj, L, W)) return KT_ERR_CUDA;
+    // per level: D, C, g, A, x; per level below the top: sep and the segment outputs
+    std::vector<double*> D(top + 1), C(top + 1), g(top + 1), A(top + 1), x(top + 1);
+    std::vector<int*> sep(top);
+    std::vector<double*> Saa(top), Sbb(top), Sba(top), ga(top), gb(top);
+    for (int l = 0; l <= top; ++l) {
+        const size_t m = plan.n[l];
+        if (mem.device(&D[l], 36 * m, W) || mem.device(&C[l], 36 * m, W) || mem.device(&g[l], 6 * m, W) || mem.device(&A[l], 36 * m, W) || mem.device(&x[l], 6 * m, W)) return KT_ERR_CUDA;
+        if (l < top) {
+            const size_t S = plan.sep[l].size() - 1;
+            if (mem.device(&sep[l], S + 1, W) || mem.device(&Saa[l], 36 * S, W) || mem.device(&Sbb[l], 36 * S, W) || mem.device(&Sba[l], 36 * S, W) ||
+                mem.device(&ga[l], 6 * S, W) || mem.device(&gb[l], 6 * S, W)) return KT_ERR_CUDA;
+            KT_CUDA(cudaMemcpyAsync(sep[l], plan.sep[l].data(), (S + 1) * sizeof(int), cudaMemcpyHostToDevice, s));
         }
-        KT_CUDA(cudaMemcpyAsync(d_f, fh, nf * sizeof(PgoFactor), cudaMemcpyHostToDevice, s));
-        KT_CUDA(cudaMemcpyAsync(d_loff, loff.data(), loff.size() * sizeof(int), cudaMemcpyHostToDevice, s));
-        if (!lidx.empty()) KT_CUDA(cudaMemcpyAsync(d_lidx, lidx.data(), lidx.size() * sizeof(int), cudaMemcpyHostToDevice, s));
-        if (L) {
-            KT_CUDA(cudaMemcpyAsync(d_ti, plan.loop_i.data(), L * sizeof(int), cudaMemcpyHostToDevice, s));
-            KT_CUDA(cudaMemcpyAsync(d_tj, plan.loop_j.data(), L * sizeof(int), cudaMemcpyHostToDevice, s));
-        }
-        if (X != poses_in) KT_CUDA(cudaMemcpyAsync(X, poses_in, 16 * (size_t)n * sizeof(double), cudaMemcpyDeviceToDevice, s));
-        KT_CUDA(cudaMemsetAsync(d_fail, 0, sizeof(int), s));
-        // chi2 and the failure flag of the current poses: the one read-back of a step.  `done` (optional) is recorded after the sum.
-        double chi2 = 0.0; int failed = 0;
-        auto linearise = [&](cudaEvent_t done) -> int {
-            pgo_linearise_kernel<<<(nf + LIN_THREADS - 1) / LIN_THREADS, LIN_THREADS, 0, s>>>(X, d_f, nf, d_E, d_JI, d_JJ, d_e2); KT_LAUNCH_CHECK();
-            pgo_sum_kernel<<<1, SUM_THREADS, 0, s>>>(d_e2, nf, d_out); KT_LAUNCH_CHECK();
-            if (done) KT_CUDA(cudaEventRecord(done, s));
-            KT_CUDA(cudaMemcpyAsync(&chi2, d_out, sizeof(double), cudaMemcpyDeviceToHost, s));
-            KT_CUDA(cudaMemcpyAsync(&failed, d_fail, sizeof(int), cudaMemcpyDeviceToHost, s));
-            KT_CUDA(cudaStreamSynchronize(s));
-            return 0;
-        };
-        // device time of each step, from the assembly to the chi2 of the updated poses (kt_pgo_report::step_ms)
-        KT_CUDA(cudaEventCreate(&ev[0])); KT_CUDA(cudaEventCreate(&ev[1]));
-        int r = linearise(0); if (r) return r;
-        double prev = chi2, step_ms = 0.0;
-        rep->chi2_initial = rep->chi2_final = prev;
-        for (int it = 0; it < 100; ++it) {
-            KT_CUDA(cudaEventRecord(ev[0], s));
-            pgo_assemble_kernel<<<(nf + 127) / 128, 128, 0, s>>>(n, nf, d_f, d_E, d_JI, d_JJ, d_loff, d_lidx, D[0], C[0], g[0], d_HL); KT_LAUNCH_CHECK();
-            for (int l = 0; l < top; ++l) {
-                const int S = (int)plan.sep[l].size() - 1, P = plan.n[l + 1];
-                pgo_segment_kernel<<<S, 32, 0, s>>>(sep[l], D[l], C[l], g[l], A[l], Saa[l], Sbb[l], Sba[l], ga[l], gb[l], d_fail); KT_LAUNCH_CHECK();
-                pgo_gather_kernel<<<(unsigned)(((size_t)P * 42 + 255) / 256), 256, 0, s>>>(P, sep[l], D[l], g[l], Saa[l], Sbb[l], Sba[l], ga[l], gb[l],
-                                                                                              D[l + 1], C[l + 1], g[l + 1]); KT_LAUNCH_CHECK();
-            }
-            pgo_dense_fill_kernel<<<(unsigned)(((size_t)N * N + 255) / 256), 256, 0, s>>>(K, D[top], C[top], d_M); KT_LAUNCH_CHECK();
-            if (L) { pgo_dense_loops_kernel<<<1, 64, 0, s>>>(K, L, d_ti, d_tj, d_HL, d_M); KT_LAUNCH_CHECK(); }
-            for (int j0 = 0; j0 < N; j0 += 6) {
-                const int T = (N - j0 - 6 + TILE - 1) / TILE, tiles = T > 0 ? T * (T + 1) / 2 : 1;
-                pgo_dense_panel_kernel<<<tiles, TILE * 8, 0, s>>>(N, j0, d_M, d_Lf, d_fail); KT_LAUNCH_CHECK();
-            }
-            KT_CUDA(cudaMemcpyAsync(x[top], g[top], (size_t)N * sizeof(double), cudaMemcpyDeviceToDevice, s));
-            pgo_dense_solve_kernel<<<1, SOLVE_THREADS, 0, s>>>(N, d_Lf, x[top], d_fail); KT_LAUNCH_CHECK();
-            for (int l = top - 1; l >= 0; --l) {
-                const int S = (int)plan.sep[l].size() - 1;
-                pgo_backsub_kernel<<<(S + 127) / 128, 128, 0, s>>>(S, sep[l], D[l], A[l], C[l], g[l], x[l + 1], x[l], d_fail); KT_LAUNCH_CHECK();
-            }
-            pgo_update_kernel<<<(n + 127) / 128, 128, 0, s>>>(n, x[0], X, d_fail); KT_LAUNCH_CHECK();
-            r = linearise(ev[1]); if (r) return r;
-            float ms = 0.f;
-            KT_CUDA(cudaEventElapsedTime(&ms, ev[0], ev[1]));
-            step_ms += ms;
-            rep->iterations = it + 1;
-            rep->step_ms = step_ms / rep->iterations;
-            if (failed) { rep->solver_failed = 1; break; }
-            const double dec = prev - chi2;
-            rep->chi2_final = chi2;
-            if (dec < 1e-3 || dec < 1e-5 * prev) break;
-            prev = chi2;
-        }
+    }
+    KT_CUDA(cudaMemcpyAsync(d_f, fh, nf * sizeof(PgoFactor), cudaMemcpyHostToDevice, s));
+    KT_CUDA(cudaMemcpyAsync(d_loff, loff.data(), loff.size() * sizeof(int), cudaMemcpyHostToDevice, s));
+    if (!lidx.empty()) KT_CUDA(cudaMemcpyAsync(d_lidx, lidx.data(), lidx.size() * sizeof(int), cudaMemcpyHostToDevice, s));
+    if (L) {
+        KT_CUDA(cudaMemcpyAsync(d_ti, plan.loop_i.data(), L * sizeof(int), cudaMemcpyHostToDevice, s));
+        KT_CUDA(cudaMemcpyAsync(d_tj, plan.loop_j.data(), L * sizeof(int), cudaMemcpyHostToDevice, s));
+    }
+    if (X != poses_in) KT_CUDA(cudaMemcpyAsync(X, poses_in, 16 * (size_t)n * sizeof(double), cudaMemcpyDeviceToDevice, s));
+    KT_CUDA(cudaMemsetAsync(d_fail, 0, sizeof(int), s));
+    // chi2 and the failure flag of the current poses: the one read-back of a step.  `done` (optional) is recorded after the sum.
+    double chi2 = 0.0; int failed = 0;
+    auto linearise = [&](cudaEvent_t done) -> int {
+        pgo_linearise_kernel<<<(nf + LIN_THREADS - 1) / LIN_THREADS, LIN_THREADS, 0, s>>>(X, d_f, nf, d_E, d_JI, d_JJ, d_e2); KT_LAUNCH_CHECK();
+        pgo_sum_kernel<<<1, SUM_THREADS, 0, s>>>(d_e2, nf, d_out); KT_LAUNCH_CHECK();
+        if (done) KT_CUDA(cudaEventRecord(done, s));
+        KT_CUDA(cudaMemcpyAsync(&chi2, d_out, sizeof(double), cudaMemcpyDeviceToHost, s));
+        KT_CUDA(cudaMemcpyAsync(&failed, d_fail, sizeof(int), cudaMemcpyDeviceToHost, s));
+        KT_CUDA(cudaStreamSynchronize(s));
         return 0;
     };
-    const int r = run();
-    cudaStreamSynchronize(s);
-    for (cudaEvent_t e : ev) if (e) cudaEventDestroy(e);
-    for (void* p : owned) cudaFree(p);
-    return r;
+    // device time of each step, from the assembly to the chi2 of the updated poses (kt_pgo_report::step_ms)
+    cudaEvent_t ev[2];
+    int r;
+    if ((r = mem.event(&ev[0], cudaEventDefault, W)) || (r = mem.event(&ev[1], cudaEventDefault, W))) return r;
+    r = linearise(0); if (r) return r;
+    double prev = chi2, step_ms = 0.0;
+    rep->chi2_initial = rep->chi2_final = prev;
+    for (int it = 0; it < 100; ++it) {
+        KT_CUDA(cudaEventRecord(ev[0], s));
+        pgo_assemble_kernel<<<(nf + 127) / 128, 128, 0, s>>>(n, nf, d_f, d_E, d_JI, d_JJ, d_loff, d_lidx, D[0], C[0], g[0], d_HL); KT_LAUNCH_CHECK();
+        for (int l = 0; l < top; ++l) {
+            const int S = (int)plan.sep[l].size() - 1, P = plan.n[l + 1];
+            pgo_segment_kernel<<<S, 32, 0, s>>>(sep[l], D[l], C[l], g[l], A[l], Saa[l], Sbb[l], Sba[l], ga[l], gb[l], d_fail); KT_LAUNCH_CHECK();
+            pgo_gather_kernel<<<(unsigned)(((size_t)P * 42 + 255) / 256), 256, 0, s>>>(P, sep[l], D[l], g[l], Saa[l], Sbb[l], Sba[l], ga[l], gb[l],
+                                                                                          D[l + 1], C[l + 1], g[l + 1]); KT_LAUNCH_CHECK();
+        }
+        pgo_dense_fill_kernel<<<(unsigned)(((size_t)N * N + 255) / 256), 256, 0, s>>>(K, D[top], C[top], d_M); KT_LAUNCH_CHECK();
+        if (L) { pgo_dense_loops_kernel<<<1, 64, 0, s>>>(K, L, d_ti, d_tj, d_HL, d_M); KT_LAUNCH_CHECK(); }
+        for (int j0 = 0; j0 < N; j0 += 6) {
+            const int T = (N - j0 - 6 + TILE - 1) / TILE, tiles = T > 0 ? T * (T + 1) / 2 : 1;
+            pgo_dense_panel_kernel<<<tiles, TILE * 8, 0, s>>>(N, j0, d_M, d_Lf, d_fail); KT_LAUNCH_CHECK();
+        }
+        KT_CUDA(cudaMemcpyAsync(x[top], g[top], (size_t)N * sizeof(double), cudaMemcpyDeviceToDevice, s));
+        pgo_dense_solve_kernel<<<1, SOLVE_THREADS, 0, s>>>(N, d_Lf, x[top], d_fail); KT_LAUNCH_CHECK();
+        for (int l = top - 1; l >= 0; --l) {
+            const int S = (int)plan.sep[l].size() - 1;
+            pgo_backsub_kernel<<<(S + 127) / 128, 128, 0, s>>>(S, sep[l], D[l], A[l], C[l], g[l], x[l + 1], x[l], d_fail); KT_LAUNCH_CHECK();
+        }
+        pgo_update_kernel<<<(n + 127) / 128, 128, 0, s>>>(n, x[0], X, d_fail); KT_LAUNCH_CHECK();
+        r = linearise(ev[1]); if (r) return r;
+        float ms = 0.f;
+        KT_CUDA(cudaEventElapsedTime(&ms, ev[0], ev[1]));
+        step_ms += ms;
+        rep->iterations = it + 1;
+        rep->step_ms = step_ms / rep->iterations;
+        if (failed) { rep->solver_failed = 1; break; }
+        const double dec = prev - chi2;
+        rep->chi2_final = chi2;
+        if (dec < 1e-3 || dec < 1e-5 * prev) break;
+        prev = chi2;
+    }
+    return 0;
 }
 
 } // namespace kt

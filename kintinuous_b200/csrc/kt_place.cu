@@ -339,26 +339,16 @@ int match_ratio(const float* db, int n_seg, int stride, const int* seg_count_dev
 int pnp_ransac(const PnpArgs& a, PnpWorkspace* ws, double* pose12, unsigned char* inliers, int* n_inliers, cudaStream_t s)
 {
     if (a.n < 3 || a.iterations < 1) { set_error("pnp_ransac: need at least 3 matches and 1 iteration"); return KT_ERR_INVALID; }
-    if (ws->cap < a.iterations) {
-        if (ws->counts) cudaFree(ws->counts);
-        if (ws->hyps) cudaFree(ws->hyps);
-        ws->counts = 0; ws->hyps = 0; ws->cap = 0;
-        KT_CUDA(cudaMalloc((void**)&ws->counts, (size_t)a.iterations * sizeof(int)));
-        KT_CUDA(cudaMalloc((void**)&ws->hyps, (size_t)a.iterations * 12 * sizeof(double)));
-        ws->cap = a.iterations;
+    const size_t it = (size_t)a.iterations;
+    int r;
+    if ((r = ws->counts.grow(it, it, "pnp inlier counts")) || (r = ws->hyps.grow(12 * it, 12 * it, "pnp hypotheses"))) return r;
+    if (!ws->counter.get()) {
+        if ((r = ws->counter.grow(1, 1, "pnp counter"))) return r;
+        KT_CUDA(cudaMemset(ws->counter.get(), 0, sizeof(unsigned int)));
     }
-    if (!ws->counter) { KT_CUDA(cudaMalloc((void**)&ws->counter, sizeof(unsigned int))); KT_CUDA(cudaMemset(ws->counter, 0, sizeof(unsigned int))); }
-    pnp_ransac_kernel<<<a.iterations, PNP_THREADS, 27 * PNP_THREADS * sizeof(double), s>>>(a, ws->counts, ws->hyps, ws->counter, pose12, inliers, n_inliers);
+    pnp_ransac_kernel<<<a.iterations, PNP_THREADS, 27 * PNP_THREADS * sizeof(double), s>>>(a, ws->counts.get(), ws->hyps.get(), ws->counter.get(), pose12, inliers, n_inliers);
     KT_LAUNCH_CHECK();
     return 0;
-}
-
-void pnp_ws_free(PnpWorkspace* ws)
-{
-    if (ws->counts) cudaFree(ws->counts);
-    if (ws->hyps) cudaFree(ws->hyps);
-    if (ws->counter) cudaFree(ws->counter);
-    *ws = PnpWorkspace();
 }
 
 int depth_to_cloud(const uint16_t* depth, int rows, int cols, const Intr& k, void* cloud, cudaStream_t s)

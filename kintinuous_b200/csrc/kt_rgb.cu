@@ -11,7 +11,7 @@
 //   computeRgbResidual / RGBResidual / residualKernel   cuda/reduce.cu:668-864
 //   rgbStep / RGBReduction / rgbKernel                  cuda/reduce.cu:423-607
 //   host half of RGBDOdometry::getIncrementalTransformation   RGBDOdometry.cpp:205-370
-// Design: no per-call cudaMalloc/cudaFree (the reference allocates the 25-tap table and the reduce
+// Design: no per-call device allocation or free (the reference allocates the 25-tap table and the reduce
 // scratch on every call, SURVEY.md section 3.2); the warp (K R K^-1, K t) of each iteration is rebuilt on the
 // device from the running estimate; the sigma of the robust weight and the Gauss-Newton solve live in the
 // reduction tails, so an iteration is 2 launches (3 with ICP) and no host round trip.  The tracker itself uses rgbd_frame_kernel:

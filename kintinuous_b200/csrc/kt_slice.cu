@@ -399,41 +399,19 @@ int grid_for(size_t n) { size_t b = (n + SL_THREADS - 1) / SL_THREADS; const siz
 // Workspace of one slice: grown on demand, owned by the caller (tracker context or operator scratch).
 int slice_ws_reserve(SliceWorkspace* ws, size_t words, size_t n_points)
 {
-    if (ws->words_cap < words) {
-        if (ws->mask) cudaFree(ws->mask);
-        if (ws->word_off) cudaFree(ws->word_off);
-        if (ws->block_tot) cudaFree(ws->block_tot);
-        ws->mask = 0; ws->word_off = 0; ws->block_tot = 0; ws->words_cap = 0;
-        const size_t w = words + words / 4 + 1024;
-        KT_CUDA(cudaMalloc((void**)&ws->mask, w * sizeof(unsigned int)));
-        KT_CUDA(cudaMalloc((void**)&ws->word_off, w * sizeof(unsigned int)));
-        KT_CUDA(cudaMalloc((void**)&ws->block_tot, ((w + SCAN_BLOCK - 1) / SCAN_BLOCK + 1) * sizeof(unsigned int)));
-        ws->words_cap = w;
+    int r;
+    if (ws->mask.capacity() < words) {      // the three word arrays grow together; mask is allocated last, so its capacity covers all three
+        ws->mask.reset(); ws->word_off.reset(); ws->block_tot.reset();
+        const size_t w = words + words / 4 + 1024, b = (w + SCAN_BLOCK - 1) / SCAN_BLOCK + 1;
+        if ((r = ws->word_off.grow(w, w, "slice word offsets")) || (r = ws->block_tot.grow(b, b, "slice scan totals")) ||
+            (r = ws->mask.grow(w, w, "slice leaf bitmap"))) return r;
     }
-    if (ws->acc_cap < n_points) {
-        if (ws->acc) cudaFree(ws->acc);
-        ws->acc = 0; ws->acc_cap = 0;
-        const size_t m = n_points + n_points / 4 + 1024;
-        KT_CUDA(cudaMalloc((void**)&ws->acc, m * sizeof(SliceAcc)));
-        ws->acc_cap = m;
-    }
-    if (!ws->bounds) {
-        KT_CUDA(cudaMalloc((void**)&ws->bounds, 8 * sizeof(unsigned int)));
-        KT_CUDA(cudaMallocHost((void**)&ws->bounds_host, 8 * sizeof(unsigned int)));
+    const size_t m = n_points + n_points / 4 + 1024;
+    if ((r = ws->acc.grow(n_points * sizeof(SliceAcc), m * sizeof(SliceAcc), "slice leaf accumulators"))) return r;
+    if (!ws->bounds_host) {
+        if ((r = ws->fixed.device(&ws->bounds, 8, "slice bounds")) || (r = ws->fixed.pinned(&ws->bounds_host, 8, "slice bounds"))) return r;
     }
     return 0;
-}
-
-void slice_ws_free(SliceWorkspace* ws)
-{
-    if (ws->mask) cudaFree(ws->mask);
-    if (ws->word_off) cudaFree(ws->word_off);
-    if (ws->block_tot) cudaFree(ws->block_tot);
-    if (ws->acc) cudaFree(ws->acc);
-    if (ws->bounds) cudaFree(ws->bounds);
-    if (ws->bounds_host) cudaFreeHost(ws->bounds_host);
-    SliceWorkspace z = {0, 0, 0, 0, 0, 0, 0, 0};
-    *ws = z;
 }
 
 namespace {
@@ -475,24 +453,24 @@ int leaf_grid(const kt_point_xyzrgb* in, size_t n, int weight_cull, float leaf, 
     g.cells = (unsigned long long)g.div_b[0] * g.div_b[1] * g.div_b[2];
     const size_t words = (size_t)((g.cells + 31) / 32);
     if ((r = slice_ws_reserve(ws, words, kept))) return r;
-    KT_CUDA(cudaMemsetAsync(ws->mask, 0, words * sizeof(unsigned int), s));
-    slice_mark_kernel<<<grid_for(n), SL_THREADS, 0, s>>>(in, (unsigned int)n, weight_cull, g, ws->mask);
+    KT_CUDA(cudaMemsetAsync(ws->mask.get(), 0, words * sizeof(unsigned int), s));
+    slice_mark_kernel<<<grid_for(n), SL_THREADS, 0, s>>>(in, (unsigned int)n, weight_cull, g, ws->mask.get());
     KT_LAUNCH_CHECK();
     const unsigned int nblocks = (unsigned int)((words + SCAN_BLOCK - 1) / SCAN_BLOCK);
-    scan_block_totals_kernel<<<nblocks, SL_THREADS, 0, s>>>(ws->mask, words, ws->block_tot);
+    scan_block_totals_kernel<<<nblocks, SL_THREADS, 0, s>>>(ws->mask.get(), words, ws->block_tot.get());
     KT_LAUNCH_CHECK();
-    scan_totals_kernel<<<1, SL_THREADS, 0, s>>>(ws->block_tot, nblocks, ws->bounds + 7);
+    scan_totals_kernel<<<1, SL_THREADS, 0, s>>>(ws->block_tot.get(), nblocks, ws->bounds + 7);
     KT_LAUNCH_CHECK();
-    scan_final_kernel<<<nblocks, SL_THREADS, 0, s>>>(ws->mask, words, ws->block_tot, ws->word_off);
+    scan_final_kernel<<<nblocks, SL_THREADS, 0, s>>>(ws->mask.get(), words, ws->block_tot.get(), ws->word_off.get());
     KT_LAUNCH_CHECK();
-    KT_CUDA(cudaMemsetAsync(ws->acc, 0, (size_t)kept * sizeof(SliceAcc), s));
-    slice_accumulate_kernel<<<grid_for(n), SL_THREADS, 0, s>>>(in, (unsigned int)n, weight_cull, g, ws->mask, ws->word_off, (SliceAcc*)ws->acc);
+    KT_CUDA(cudaMemsetAsync(ws->acc.get(), 0, (size_t)kept * sizeof(SliceAcc), s));
+    slice_accumulate_kernel<<<grid_for(n), SL_THREADS, 0, s>>>(in, (unsigned int)n, weight_cull, g, ws->mask.get(), ws->word_off.get(), (SliceAcc*)ws->acc.get());
     KT_LAUNCH_CHECK();
     KT_CUDA(cudaMemcpyAsync(ws->bounds_host + 7, ws->bounds + 7, sizeof(unsigned int), cudaMemcpyDeviceToHost, s));
     KT_CUDA(cudaStreamSynchronize(s));
     const unsigned int n_out = ws->bounds_host[7];
     if ((size_t)n_out > capacity) { set_error("%s: %u processed points do not fit the output capacity %zu", who, n_out, capacity); return KT_ERR_CAPACITY; }
-    slice_centroid_kernel<<<div_up((int)n_out, SL_THREADS), SL_THREADS, 0, s>>>((const SliceAcc*)ws->acc, n_out, (unsigned int)capacity, out);
+    slice_centroid_kernel<<<div_up((int)n_out, SL_THREADS), SL_THREADS, 0, s>>>((const SliceAcc*)ws->acc.get(), n_out, (unsigned int)capacity, out);
     KT_LAUNCH_CHECK();
     *gout = g; *n_out_p = n_out;
     return 0;
@@ -578,7 +556,7 @@ int process_slice(const void* points_dev, size_t n, int weight_cull, float leaf,
         int blocks = div_up((int)n_out, warps_per_block);
         const int cap = device_info().sm_count * 16;
         if (blocks > cap) blocks = cap;
-        slice_normals_kernel<<<blocks, NRM_THREADS, 0, s>>>(out, (const SliceAcc*)ws->acc, n_out, k_search, g, ws->mask, ws->word_off);
+        slice_normals_kernel<<<blocks, NRM_THREADS, 0, s>>>(out, (const SliceAcc*)ws->acc.get(), n_out, k_search, g, ws->mask.get(), ws->word_off.get());
         KT_LAUNCH_CHECK();
     }
     if (count) *count = n_out;
@@ -601,7 +579,7 @@ int cloud_fitness(const void* src, size_t n_src, const void* dst, size_t n_dst, 
     if (ns == 0 || nd == 0) return 0;
     float* Td = (float*)(d2_dev + capacity + 1);
     KT_CUDA(cudaMemcpyAsync(Td, T12, 12 * sizeof(float), cudaMemcpyHostToDevice, s));
-    cloud_nn_kernel<<<div_up((int)ns, SL_THREADS), SL_THREADS, 0, s>>>(so, ns, Td, dso, nd, gd, ws_dst->mask, ws_dst->word_off, d2_dev);
+    cloud_nn_kernel<<<div_up((int)ns, SL_THREADS), SL_THREADS, 0, s>>>(so, ns, Td, dso, nd, gd, ws_dst->mask.get(), ws_dst->word_off.get(), d2_dev);
     KT_LAUNCH_CHECK();
     sum_fixed_kernel<<<1, SL_THREADS, 0, s>>>(d2_dev, ns, d2_dev + capacity);
     KT_LAUNCH_CHECK();

@@ -298,35 +298,22 @@ static SurfGeom surf_geom(int rows, int cols)
 
 int surf_ws_reserve(SurfWorkspace* ws, int rows, int cols)
 {
-    if (ws->rows == rows && ws->cols == cols && ws->integral) return 0;
-    surf_ws_free(ws);
+    if (ws->rows == rows && ws->cols == cols) return 0;
+    *ws = SurfWorkspace();
     const SurfGeom g = surf_geom(rows, cols);
     size_t nresp = 0;
     for (int o = 0; o < SURF_OCT; ++o) nresp += (size_t)SURF_LAY * g.grid_r[o] * g.grid_c[o];
-    KT_CUDA(cudaMalloc((void**)&ws->integral, (size_t)(rows + 1) * (cols + 1) * sizeof(int)));
-    KT_CUDA(cudaMalloc((void**)&ws->resp, nresp * sizeof(float)));
     const size_t nc = g.ncells;
-    KT_CUDA(cudaMalloc((void**)&ws->cand, nc * sizeof(SurfCand)));
-    KT_CUDA(cudaMalloc((void**)&ws->keys, nc * 2 * sizeof(unsigned long long)));
-    KT_CUDA(cudaMalloc((void**)&ws->idx, nc * 2 * sizeof(unsigned int)));
-    KT_CUDA(cudaMalloc((void**)&ws->n_cand, sizeof(unsigned int)));
     size_t tmp = 0;
     cub::DeviceRadixSort::SortPairs(nullptr, tmp, (unsigned long long*)0, (unsigned long long*)0, (unsigned int*)0, (unsigned int*)0, (int)nc);
-    KT_CUDA(cudaMalloc(&ws->tmp, tmp));
-    ws->tmp_bytes = tmp; ws->rows = rows; ws->cols = cols;
+    SurfCand* cand = 0;
+    int r;
+    if ((r = ws->mem.device(&ws->integral, (size_t)(rows + 1) * (cols + 1), "surf integral image")) ||
+        (r = ws->mem.device(&ws->resp, nresp, "surf responses")) || (r = ws->mem.device(&cand, nc, "surf candidates")) ||
+        (r = ws->mem.device(&ws->keys, nc * 2, "surf sort keys")) || (r = ws->mem.device(&ws->idx, nc * 2, "surf sort indices")) ||
+        (r = ws->mem.device(&ws->n_cand, 1, "surf candidate count")) || (r = ws->mem.device(&ws->tmp, tmp, "surf sort storage"))) return r;
+    ws->cand = cand; ws->tmp_bytes = tmp; ws->rows = rows; ws->cols = cols;
     return 0;
-}
-
-void surf_ws_free(SurfWorkspace* ws)
-{
-    if (ws->integral) cudaFree(ws->integral);
-    if (ws->resp) cudaFree(ws->resp);
-    if (ws->cand) cudaFree(ws->cand);
-    if (ws->keys) cudaFree(ws->keys);
-    if (ws->idx) cudaFree(ws->idx);
-    if (ws->n_cand) cudaFree(ws->n_cand);
-    if (ws->tmp) cudaFree(ws->tmp);
-    *ws = SurfWorkspace();
 }
 
 int surf(const uint8_t* rgb, int rows, int cols, float threshold, int max_features, float* kp, float* desc, int* n_out, SurfWorkspace* ws, cudaStream_t s)

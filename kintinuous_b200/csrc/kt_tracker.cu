@@ -20,6 +20,7 @@
 #include "kt_place.hpp"
 #include <cstdlib>
 #include "../../include/kintinuous_b200.h"
+#include <memory>
 #include <vector>
 #include <unordered_map>
 #include <cstring>
@@ -89,11 +90,11 @@ static Mat33 to_mat33(const float* m) { Mat33 r; r.r0 = make_float3(m[0], m[1], 
 // processFrame (KintinuousTracker.cpp:1166, containers/device_memory.cpp:146-157).
 struct SliceRec { int dimension; kt_point_xyzrgb* points; size_t count; kt_point_xyzrgbnormal* processed; size_t processed_count; bool has_processed;
                   kt_mesh_vertex* mesh_verts; uint32_t* mesh_tris; size_t mesh_nv, mesh_nt; bool has_mesh;
-                  cudaEvent_t ready; float camera_t[3]; float camera_R[9]; uint64_t utime; };
+                  Event ready; float camera_t[3]; float camera_R[9]; uint64_t utime; };
 
-// Pinned host memory handed out in slabs (one cudaHostAlloc per 64 MB, not per slice); everything is released together by kt_reset.
+// Pinned host memory handed out in slabs (one allocation per 64 MB, not per slice); kt_reset rewinds it, the slabs live as long as it.
 struct PinnedArena {
-    std::vector<std::pair<char*, size_t> > chunks; size_t chunk_used; size_t current;
+    Allocations slabs; std::vector<std::pair<char*, size_t> > chunks; size_t chunk_used; size_t current;
     PinnedArena() : chunk_used(0), current(0) {}
     void* alloc(size_t bytes)
     {
@@ -101,9 +102,9 @@ struct PinnedArena {
         while (current < chunks.size() && chunk_used + bytes > chunks[current].second) { ++current; chunk_used = 0; }
         if (current >= chunks.size()) {
             const size_t sz = std::max(bytes, (size_t)64 << 20);
-            void* q = 0;
-            if (cudaHostAlloc(&q, sz, cudaHostAllocDefault) != cudaSuccess) return 0;
-            chunks.push_back(std::make_pair((char*)q, sz));
+            char* q = 0;
+            if (slabs.pinned(&q, sz, "a pinned arena slab")) return 0;
+            chunks.push_back(std::make_pair(q, sz));
             current = chunks.size() - 1; chunk_used = 0;
         }
         void* r = chunks[current].first + chunk_used;
@@ -111,7 +112,6 @@ struct PinnedArena {
         return r;
     }
     void rewind() { current = 0; chunk_used = 0; }
-    void release() { for (auto& c : chunks) cudaFreeHost(c.first); chunks.clear(); rewind(); }
 };
 
 // what the host reads back after the odometry of a frame
@@ -120,6 +120,7 @@ struct OdomResult { float Rcurr[9]; float tcurr[3]; int timeout; unsigned int se
 // Place recognition (kt_set_loop_detection / kt_detect_loops): keyframes' raw depth, SURF keypoints / descriptors and their 3-D points, captured on
 // `stream` (the frame path never waits for it on the host), and the scratch of the detection chain.  Allocated only while detection is on.
 struct PlaceStore {
+    Allocations mem;
     kt_loop_detection_params p;
     int rows, cols, maxK, maxF;
     cudaStream_t stream; cudaEvent_t ev_input, ev_copied;
@@ -136,21 +137,8 @@ struct PlaceStore {
     OdomState* state; unsigned long long* xwords; float* trace;
     kt_point_xyzrgb* cloud[2]; kt_point_xyzrgbnormal* cent[2]; double* d2fit; SliceWorkspace ws[2];
     std::vector<std::vector<float> > in_new, in_old;      // inliers of the results of the last kt_detect_loops
-    std::vector<void*> allocs;
-    template <class T> int alloc(T** q, size_t n) { void* v = 0; KT_CUDA(cudaMalloc(&v, n ? n * sizeof(T) : 1)); allocs.push_back(v); *q = (T*)v; return 0; }
+    ~PlaceStore() { if (stream) cudaStreamSynchronize(stream); }
 };
-
-static void place_free(PlaceStore* ps)
-{
-    if (!ps) return;
-    if (ps->stream) { cudaStreamSynchronize(ps->stream); cudaStreamDestroy(ps->stream); }
-    if (ps->ev_input) cudaEventDestroy(ps->ev_input);
-    if (ps->ev_copied) cudaEventDestroy(ps->ev_copied);
-    if (ps->nfeat_host) cudaFreeHost(ps->nfeat_host);
-    surf_ws_free(&ps->surf_ws); pnp_ws_free(&ps->pnp_ws); slice_ws_free(&ps->ws[0]); slice_ws_free(&ps->ws[1]);
-    for (void* q : ps->allocs) cudaFree(q);
-    delete ps;
-}
 
 } // namespace kt
 
@@ -188,16 +176,16 @@ struct kt_ctx {
     OdomState* state; float* partials; int* ipartials; float* trace_dev; float* pose12_dev; long long* prof_dev;
     kt_point_xyzrgb* cloud_dev; unsigned int* counter_dev; size_t cloud_capacity; size_t cloud_count;
     // slice hand-off: pinned arena, asynchronous download on stream_slices; ev_cloud_free = the last download has left cloud_dev / proc_dev
-    PinnedArena* slice_arena; cudaStream_t stream_slices; cudaEvent_t ev_cloud_ready, ev_cloud_free; bool cloud_busy;
+    PinnedArena slice_arena; cudaStream_t stream_slices; cudaEvent_t ev_cloud_ready, ev_cloud_free; bool cloud_busy;
     // CloudSliceProcessor on the device (kt_slice.cu): weight cull + voxel grid + normals of every slice before it leaves the GPU
-    int slice_processing, slice_weight_cull; SliceWorkspace slice_ws; kt_point_xyzrgbnormal* proc_dev; size_t proc_count;
+    int slice_processing, slice_weight_cull; SliceWorkspace slice_ws; DeviceBuffer<kt_point_xyzrgbnormal> proc; size_t proc_count;
     // marching cubes of every slice's box before it is cleared (kt_mesh.cu); buffers grow at a shift, downloaded with the slice
-    int slice_meshing, mesh_weight_cull; MeshWorkspace mesh_ws; kt_mesh_vertex* mesh_verts_dev; uint32_t* mesh_tris_dev;
-    size_t mesh_verts_cap, mesh_tris_cap, mesh_nv, mesh_nt;
+    int slice_meshing, mesh_weight_cull; MeshWorkspace mesh_ws; DeviceBuffer<kt_mesh_vertex> mesh_verts; DeviceBuffer<uint32_t> mesh_tris;
+    size_t mesh_nv, mesh_nt;
     // the map as deformed by the last kt_deform_map (kt_deform.cu): one record per slice recorded before that call, in its own pinned
     // arena, or the slice's own buffers when the call left the map unchanged
     struct Deformed { kt_point_xyzrgbnormal* processed; kt_mesh_vertex* mesh_verts; };
-    std::vector<Deformed> deformed; PinnedArena* deform_arena;
+    std::vector<Deformed> deformed; PinnedArena deform_arena;
     // loop closure (kt_close_loop, kt_pgo.cu): the accepted loops with their inliers, and the optimised nodes of the last accepted one
     struct Loop { uint64_t time1, time2; double C[16]; std::vector<float> in1, in2; };
     std::vector<Loop> loops; std::vector<kt_dense_pose> pgo_nodes;
@@ -214,7 +202,7 @@ struct kt_ctx {
     // timing
     bool timing; cudaEvent_t ev[7]; float stage_ms[6]; cudaEvent_t ev_icp[2]; cudaEvent_t ev_krn[4]; cudaEvent_t ev_span[2];     // ev_krn: integrate / raycast launches alone (without the cross-GPU barriers the stage timers include)
     long long launches_at_create;
-    std::vector<void*> allocs;
+    Allocations mem;           // device and pinned buffers, events and streams created with the context
     // ONE volume shared by `world` GPUs (one process per GPU; peers' arenas are mapped through CUDA IPC): TSDF plane replicated, colour /
     // weight plane sharded block-cyclically by storage z (VolumeView, kt_ops.h)
     int world, rank, local_planes, mg_block;
@@ -225,23 +213,21 @@ struct kt_ctx {
     unsigned int** peer_flags_dev; unsigned int epoch; int* mg_error_dev; int* mg_error_host;
     VolumeView vv;
     float last_int_Rinv[9], last_int_t[3]; int last_int_wrap[3];       // arguments of the last integration (kt_debug_last_integrate)
-    uint8_t* view_dev;                                                  // GUI taps: shaded image, colour image, model depth (allocated on first use)
-    PlaceStore* place;                                                  // loop detection (null while it is off)
+    DeviceBuffer<uint8_t> view;                                         // GUI taps: shaded image, colour image, model depth (allocated on first use)
+    std::unique_ptr<PlaceStore> place;                                  // loop detection (null while it is off)
+    // what member destructors cannot do: wait for the streams, unmap the peers' arenas, close the pose log
+    ~kt_ctx()
+    {
+        cudaSetDevice(cfg.device);
+        for (cudaStream_t s : {stream, stream_copy, stream_slices}) if (s) cudaStreamSynchronize(s);
+        for (int g = 0; g < MAX_GPUS; ++g) if (peer_arena[g] && peer_arena[g] != arena) cudaIpcCloseMemHandle(peer_arena[g]);
+        if (pose_log) fclose(pose_log);
+    }
 };
 
 namespace {
 
 const int MAX_TRACE_ITERS = 64;
-
-template <class T> int dev_alloc(kt_ctx* c, T** p, size_t count)
-{
-    void* q = 0;
-    const size_t bytes = count * sizeof(T);
-    KT_CUDA(cudaMalloc(&q, bytes ? bytes : 1));
-    c->allocs.push_back(q);
-    *p = (T*)q;
-    return 0;
-}
 
 void vwrap_copy(const kt_ctx* c, int* w)       // KintinuousTracker::vWrapCopyUpdate (.cpp:1075-1085)
 {
@@ -279,24 +265,12 @@ int mesh_box(kt_ctx* c, const int* vWrapCopy, const int* lo, const int* hi)
     a.minX = lo[0]; a.maxX = hi[0]; a.minY = lo[1]; a.maxY = hi[1]; a.minZ = lo[2]; a.maxZ = hi[2]; a.weight_cull = c->mesh_weight_cull;
     size_t nv = 0, nt = 0;
     int r = mesh_count(a, &c->mesh_ws, &nv, &nt, c->stream); if (r) return r;
-    if (nv > c->mesh_verts_cap || nt > c->mesh_tris_cap) {
+    if (nv > c->mesh_verts.capacity() || 3 * nt > c->mesh_tris.capacity()) {
         KT_CUDA(cudaStreamSynchronize(c->stream_slices));
-        if (nv > c->mesh_verts_cap) {
-            if (c->mesh_verts_dev) cudaFree(c->mesh_verts_dev);
-            c->mesh_verts_dev = 0; c->mesh_verts_cap = 0;
-            const size_t want = nv + nv / 4 + 1024;
-            KT_CUDA(cudaMalloc((void**)&c->mesh_verts_dev, want * sizeof(kt_mesh_vertex)));
-            c->mesh_verts_cap = want;
-        }
-        if (nt > c->mesh_tris_cap) {
-            if (c->mesh_tris_dev) cudaFree(c->mesh_tris_dev);
-            c->mesh_tris_dev = 0; c->mesh_tris_cap = 0;
-            const size_t want = nt + nt / 4 + 1024;
-            KT_CUDA(cudaMalloc((void**)&c->mesh_tris_dev, want * 3 * sizeof(uint32_t)));
-            c->mesh_tris_cap = want;
-        }
+        if ((r = c->mesh_verts.grow(nv, nv + nv / 4 + 1024, "slice mesh vertices")) ||
+            (r = c->mesh_tris.grow(3 * nt, 3 * (nt + nt / 4 + 1024), "slice mesh triangles"))) return r;
     }
-    r = mesh_emit(a, &c->mesh_ws, nv, c->mesh_verts_dev, c->mesh_tris_dev, c->stream); if (r) return r;
+    r = mesh_emit(a, &c->mesh_ws, nv, c->mesh_verts.get(), c->mesh_tris.get(), c->stream); if (r) return r;
     c->mesh_nv = nv; c->mesh_nt = nt;
     return 0;
 }
@@ -307,49 +281,48 @@ int mesh_box(kt_ctx* c, const int* vWrapCopy, const int* lo, const int* hi)
 // device first (kt_slice.cu) and both clouds are handed out.
 int push_slice(kt_ctx* c, int dimension)
 {
-    SliceRec s; s.dimension = dimension; s.points = 0; s.count = c->cloud_count; s.processed = 0; s.processed_count = 0; s.has_processed = false; s.ready = 0;
+    SliceRec s; s.dimension = dimension; s.points = 0; s.count = c->cloud_count; s.processed = 0; s.processed_count = 0; s.has_processed = false;
     s.has_mesh = c->slice_meshing != 0; s.mesh_verts = 0; s.mesh_tris = 0;
     s.mesh_nv = s.has_mesh ? c->mesh_nv : 0; s.mesh_nt = s.has_mesh ? c->mesh_nt : 0;
     c->proc_count = 0;
     if (c->slice_processing && c->cloud_count) {
-        if (!c->proc_dev) { void* q = 0; KT_CUDA(cudaMalloc(&q, c->cloud_capacity * sizeof(kt_point_xyzrgbnormal))); c->allocs.push_back(q); c->proc_dev = (kt_point_xyzrgbnormal*)q; }
-        int r = process_slice(c->cloud_dev, c->cloud_count, c->slice_weight_cull, c->voxel, 20, c->proc_dev, c->cloud_capacity, &c->proc_count, &c->slice_ws, c->stream);
+        int r = c->proc.grow(c->cloud_capacity, c->cloud_capacity, "processed slice");
+        if (!r) r = process_slice(c->cloud_dev, c->cloud_count, c->slice_weight_cull, c->voxel, 20, c->proc.get(), c->cloud_capacity, &c->proc_count, &c->slice_ws, c->stream);
         if (r) return r;
     }
     s.has_processed = c->slice_processing != 0;
     s.processed_count = c->proc_count;
     if (c->cloud_count || s.mesh_nv) {
-        if (c->cloud_count) s.points = (kt_point_xyzrgb*)c->slice_arena->alloc(c->cloud_count * sizeof(kt_point_xyzrgb));
-        if (c->proc_count) s.processed = (kt_point_xyzrgbnormal*)c->slice_arena->alloc(c->proc_count * sizeof(kt_point_xyzrgbnormal));
-        if (s.mesh_nv) s.mesh_verts = (kt_mesh_vertex*)c->slice_arena->alloc(s.mesh_nv * sizeof(kt_mesh_vertex));
-        if (s.mesh_nt) s.mesh_tris = (uint32_t*)c->slice_arena->alloc(s.mesh_nt * 3 * sizeof(uint32_t));
+        if (c->cloud_count) s.points = (kt_point_xyzrgb*)c->slice_arena.alloc(c->cloud_count * sizeof(kt_point_xyzrgb));
+        if (c->proc_count) s.processed = (kt_point_xyzrgbnormal*)c->slice_arena.alloc(c->proc_count * sizeof(kt_point_xyzrgbnormal));
+        if (s.mesh_nv) s.mesh_verts = (kt_mesh_vertex*)c->slice_arena.alloc(s.mesh_nv * sizeof(kt_mesh_vertex));
+        if (s.mesh_nt) s.mesh_tris = (uint32_t*)c->slice_arena.alloc(s.mesh_nt * 3 * sizeof(uint32_t));
         if ((c->cloud_count && !s.points) || (c->proc_count && !s.processed) || (s.mesh_nv && !s.mesh_verts) || (s.mesh_nt && !s.mesh_tris)) {
             set_error("pinned host memory for a slice of %zu points", c->cloud_count); return KT_ERR_CUDA;
         }
-        KT_CUDA(cudaEventCreateWithFlags(&s.ready, cudaEventDisableTiming));
+        int r = make_event(&s.ready, cudaEventDisableTiming, "slice download"); if (r) return r;
         KT_CUDA(cudaEventRecord(c->ev_cloud_ready, c->stream));
         KT_CUDA(cudaStreamWaitEvent(c->stream_slices, c->ev_cloud_ready, 0));
         if (c->cloud_count) KT_CUDA(cudaMemcpyAsync(s.points, c->cloud_dev, c->cloud_count * sizeof(kt_point_xyzrgb), cudaMemcpyDeviceToHost, c->stream_slices));
-        if (c->proc_count) KT_CUDA(cudaMemcpyAsync(s.processed, c->proc_dev, c->proc_count * sizeof(kt_point_xyzrgbnormal), cudaMemcpyDeviceToHost, c->stream_slices));
-        if (s.mesh_nv) KT_CUDA(cudaMemcpyAsync(s.mesh_verts, c->mesh_verts_dev, s.mesh_nv * sizeof(kt_mesh_vertex), cudaMemcpyDeviceToHost, c->stream_slices));
-        if (s.mesh_nt) KT_CUDA(cudaMemcpyAsync(s.mesh_tris, c->mesh_tris_dev, s.mesh_nt * 3 * sizeof(uint32_t), cudaMemcpyDeviceToHost, c->stream_slices));
-        KT_CUDA(cudaEventRecord(s.ready, c->stream_slices));
+        if (c->proc_count) KT_CUDA(cudaMemcpyAsync(s.processed, c->proc.get(), c->proc_count * sizeof(kt_point_xyzrgbnormal), cudaMemcpyDeviceToHost, c->stream_slices));
+        if (s.mesh_nv) KT_CUDA(cudaMemcpyAsync(s.mesh_verts, c->mesh_verts.get(), s.mesh_nv * sizeof(kt_mesh_vertex), cudaMemcpyDeviceToHost, c->stream_slices));
+        if (s.mesh_nt) KT_CUDA(cudaMemcpyAsync(s.mesh_tris, c->mesh_tris.get(), s.mesh_nt * 3 * sizeof(uint32_t), cudaMemcpyDeviceToHost, c->stream_slices));
+        KT_CUDA(cudaEventRecord(s.ready.get(), c->stream_slices));
         KT_CUDA(cudaEventRecord(c->ev_cloud_free, c->stream_slices));
         c->cloud_busy = true;
     }
     for (int i = 0; i < 3; ++i) s.camera_t[i] = c->currentGlobalCamera[i];
     for (int i = 0; i < 9; ++i) s.camera_R[i] = c->rmats.back().m[i];
     s.utime = c->current_utime;
-    c->slices.push_back(s);
+    c->slices.push_back(std::move(s));
     return 0;
 }
 
 void drop_slices(kt_ctx* c)
 {
     if (c->stream_slices) cudaStreamSynchronize(c->stream_slices);
-    for (auto& s : c->slices) if (s.ready) cudaEventDestroy(s.ready);
     c->slices.clear();
-    if (c->slice_arena) c->slice_arena->rewind();
+    c->slice_arena.rewind();
     c->cloud_busy = false;
 }
 
@@ -540,7 +513,7 @@ void record_dense_pose(kt_ctx* c, bool first, bool keyframe)
 int place_capture(kt_ctx* c, bool first, bool* keyframe)
 {
     *keyframe = false;
-    PlaceStore* ps = c->place;
+    PlaceStore* ps = c->place.get();
     if (!ps) return 0;
     const float* R = c->rmats.back().m;
     const bool kf = first || ps->times.empty() || c->shifted_last > 0 || place_is_keyframe(R, ps->lastR, c->currentGlobalCamera, ps->lastG);
@@ -720,7 +693,7 @@ int kt_reset(kt_ctx* c)
     for (int i = 0; i < 3; ++i) { c->voxelWrap[i] = 0; c->currentGlobalCamera[i] = c->volumeBasis[i] - c->size * 0.5f; }
     drop_slices(c);
     c->deformed.clear();
-    if (c->deform_arena) c->deform_arena->rewind();
+    c->deform_arena.rewind();
     c->loops.clear(); c->pgo_nodes.clear();
     std::memset(&c->map_corr, 0, sizeof(c->map_corr));
     if (c->place) {                              // reset(): the place-recognition buffer starts again (.cpp:290-298)
@@ -762,7 +735,8 @@ int kt_create(const kt_config* cfg, kt_ctx** out)
     }
     if (!kt_cuda_available()) { set_error("kt_create: no CUDA device (this library has no CPU path)"); return KT_ERR_CUDA; }
     KT_CUDA(cudaSetDevice(cfg->device));
-    kt_ctx* c = new kt_ctx();
+    std::unique_ptr<kt_ctx> owner(new kt_ctx());
+    kt_ctx* c = owner.get();
     c->cfg = *cfg;
     c->launches_at_create = g_launches.load();
     if (c->cfg.cloud_capacity <= 0) c->cfg.cloud_capacity = 3 * cfg->rows * cfg->cols;          // KintinuousTracker.cpp:77
@@ -782,14 +756,14 @@ int kt_create(const kt_config* cfg, kt_ctx** out)
         if (const char* e = getenv("KT_ODOM_ITERATIONS")) {
             int v[4];
             if (sscanf(e, "%d,%d,%d,%d", &v[0], &v[1], &v[2], &v[3]) != 4 || v[0] < 0 || v[1] < 0 || v[2] < 0 || v[3] < 0) {
-                delete c; set_error("kt_create: KT_ODOM_ITERATIONS must be four non-negative integers i0,i1,i2,i3"); return KT_ERR_INVALID; }
+                set_error("kt_create: KT_ODOM_ITERATIONS must be four non-negative integers i0,i1,i2,i3"); return KT_ERR_INVALID; }
             for (int i = 0; i < 4; ++i) c->iterations[i] = v[i];
         }
     }
-    int r = 0;
-#define KT_TRY(x) do { r = (x); if (r) { kt_destroy(c); return r; } } while (0)
-    r = kt::cuda_check(cudaStreamCreateWithFlags(&c->stream, cudaStreamNonBlocking), "stream", __FILE__, __LINE__);
-    if (r) { delete c; return r; }
+    const char* W = "kt_create";
+    auto dev = [&](auto** p, size_t n) { return c->mem.device(p, n, W); };
+    auto event = [&](cudaEvent_t* e, unsigned int flags) { return c->mem.event(e, flags, W); };
+    if (c->mem.stream(&c->stream, W)) return KT_ERR_CUDA;
     const size_t P = (size_t)cfg->rows * cfg->cols;
     {   // shared arena: local volume slab, model maps, raycast colour, barrier flags -- one allocation, one IPC handle
         c->world = cfg->world > 1 ? cfg->world : 1; c->rank = cfg->world > 1 ? cfg->rank : 0;
@@ -812,10 +786,10 @@ int kt_create(const kt_config* cfg, kt_ctx** out)
         c->off_flags = off; off = al(off + 256);
         c->off_xwords = off; off = al(off + odom_exchange_words() * sizeof(unsigned long long));      // in the arena so that peers can add to them
         c->arena_bytes = off;
-        KT_TRY(dev_alloc(c, &c->arena, off));
-        KT_TRY(kt::cuda_check(cudaMemset(c->arena + c->off_flags, 0, 256), "memset", __FILE__, __LINE__));
+        if (dev(&c->arena, off)) return KT_ERR_CUDA;
+        KT_CUDA(cudaMemset(c->arena + c->off_flags, 0, 256));
         c->xwords_dev = (unsigned long long*)(c->arena + c->off_xwords);
-        KT_TRY(kt::cuda_check(cudaMemset(c->xwords_dev, 0, odom_exchange_words() * sizeof(unsigned long long)), "memset", __FILE__, __LINE__)); c->xwords_clean = true;
+        KT_CUDA(cudaMemset(c->xwords_dev, 0, odom_exchange_words() * sizeof(unsigned long long))); c->xwords_clean = true;
         c->split_icp = c->world > 1 && getenv("KT_MG_SPLIT_ICP") != nullptr;
         c->tsdf = (int16_t*)(c->arena + c->off_tsdf); c->color = c->arena + c->off_color;
         for (int g = 0; g < MAX_GPUS; ++g) c->peer_arena[g] = c->arena;
@@ -825,100 +799,67 @@ int kt_create(const kt_config* cfg, kt_ctx** out)
         c->vv.world = c->world; c->vv.rank = c->rank;
         c->vv.bshift = 0; { int t = c->mg_block; while (t > 1) { t >>= 1; ++c->vv.bshift; } }
         c->vv.nshift = 0; { int t = c->world; while (t > 1) { t >>= 1; ++c->vv.nshift; } }
-        KT_TRY(dev_alloc(c, &c->peer_flags_dev, (size_t)MAX_GPUS)); 
+        if (dev(&c->peer_flags_dev, (size_t)MAX_GPUS)) return KT_ERR_CUDA;
         // the barrier's time-out flag lives in MAPPED host memory: the kernel writes it in place, the host reads it with the pose (no copy)
-        KT_TRY(kt::cuda_check(cudaHostAlloc((void**)&c->mg_error_host, sizeof(int), cudaHostAllocMapped), "mapped", __FILE__, __LINE__)); *c->mg_error_host = 0;
-        KT_TRY(kt::cuda_check(cudaHostGetDevicePointer((void**)&c->mg_error_dev, c->mg_error_host, 0), "mapped alias", __FILE__, __LINE__));
+        if (c->mem.mapped(&c->mg_error_host, 1, W)) return KT_ERR_CUDA; *c->mg_error_host = 0;
+        KT_CUDA(cudaHostGetDevicePointer((void**)&c->mg_error_dev, c->mg_error_host, 0));
     }
-    KT_TRY(dev_alloc(c, &c->depth_raw, P)); KT_TRY(dev_alloc(c, &c->rgb, P * 3));
-    KT_TRY(dev_alloc(c, &c->depth_alt, P)); KT_TRY(dev_alloc(c, &c->rgb_alt, P * 3)); c->pf_valid = false; c->pf_depth = c->pf_rgb = 0;
-    KT_TRY(kt::cuda_check(cudaStreamCreateWithFlags(&c->stream_copy, cudaStreamNonBlocking), "stream_copy", __FILE__, __LINE__));
-    KT_TRY(kt::cuda_check(cudaEventCreateWithFlags(&c->ev_prefetch, cudaEventDisableTiming), "event", __FILE__, __LINE__));
-    for (int i = 0; i < 2; ++i) KT_TRY(kt::cuda_check(cudaEventCreateWithFlags(&c->ev_done[i], cudaEventDisableTiming), "event", __FILE__, __LINE__));
-    KT_TRY(kt::cuda_check(cudaEventCreateWithFlags(&c->ev_maps, cudaEventDisableTiming), "event", __FILE__, __LINE__)); c->maps_on_stream = false;
+    if (dev(&c->depth_raw, P) || dev(&c->rgb, P * 3)) return KT_ERR_CUDA;
+    if (dev(&c->depth_alt, P) || dev(&c->rgb_alt, P * 3)) return KT_ERR_CUDA; c->pf_valid = false; c->pf_depth = c->pf_rgb = 0;
+    if (c->mem.stream(&c->stream_copy, W)) return KT_ERR_CUDA;
+    if (event(&c->ev_prefetch, cudaEventDisableTiming)) return KT_ERR_CUDA;
+    for (int i = 0; i < 2; ++i) if (event(&c->ev_done[i], cudaEventDisableTiming)) return KT_ERR_CUDA;
+    if (event(&c->ev_maps, cudaEventDisableTiming)) return KT_ERR_CUDA; c->maps_on_stream = false;
     c->last_parity = 0;
     for (int l = 0; l < LEVELS; ++l) {
         size_t Pl = P >> (2 * l);
-        KT_TRY(dev_alloc(c, &c->depths_curr[l], Pl));
+        if (dev(&c->depths_curr[l], Pl)) return KT_ERR_CUDA;
         c->vmaps_g_prev[l] = (float*)(c->arena + c->off_vmap[l]); c->nmaps_g_prev[l] = (float*)(c->arena + c->off_nmap[l]);
-        KT_TRY(dev_alloc(c, &c->vmaps_curr[l], Pl * 3)); KT_TRY(dev_alloc(c, &c->nmaps_curr[l], Pl * 3));
-        KT_TRY(dev_alloc(c, &c->depths_alt[l], Pl)); KT_TRY(dev_alloc(c, &c->vmaps_alt[l], Pl * 3)); KT_TRY(dev_alloc(c, &c->nmaps_alt[l], Pl * 3));
+        if (dev(&c->vmaps_curr[l], Pl * 3) || dev(&c->nmaps_curr[l], Pl * 3)) return KT_ERR_CUDA;
+        if (dev(&c->depths_alt[l], Pl) || dev(&c->vmaps_alt[l], Pl * 3) || dev(&c->nmaps_alt[l], Pl * 3)) return KT_ERR_CUDA;
         c->lastDepth[l] = c->nextDepth[l] = 0; c->lastImage[l] = c->nextImage[l] = 0; c->nextdIdx[l] = c->nextdIdy[l] = 0; c->pointClouds[l] = 0; c->corresImg[l] = 0;
         if (cfg->odometry != 0) {
-            KT_TRY(dev_alloc(c, &c->lastDepth[l], Pl)); KT_TRY(dev_alloc(c, &c->nextDepth[l], Pl));
-            KT_TRY(dev_alloc(c, &c->lastImage[l], Pl)); KT_TRY(dev_alloc(c, &c->nextImage[l], Pl));
-            KT_TRY(dev_alloc(c, &c->nextdIdx[l], Pl)); KT_TRY(dev_alloc(c, &c->nextdIdy[l], Pl));
-            KT_TRY(dev_alloc(c, &c->pointClouds[l], Pl * 3));
-            uint8_t* ci = 0; KT_TRY(dev_alloc(c, &ci, Pl * 16)); c->corresImg[l] = ci;
+            if (dev(&c->lastDepth[l], Pl) || dev(&c->nextDepth[l], Pl)) return KT_ERR_CUDA;
+            if (dev(&c->lastImage[l], Pl) || dev(&c->nextImage[l], Pl)) return KT_ERR_CUDA;
+            if (dev(&c->nextdIdx[l], Pl) || dev(&c->nextdIdy[l], Pl)) return KT_ERR_CUDA;
+            if (dev(&c->pointClouds[l], Pl * 3)) return KT_ERR_CUDA;
+            uint8_t* ci = 0; if (dev(&ci, Pl * 16)) return KT_ERR_CUDA; c->corresImg[l] = ci;
         }
     }
-    c->vmap_curr_color = c->arena + c->off_vcol; KT_TRY(dev_alloc(c, &c->depth_scaled, P)); KT_TRY(dev_alloc(c, &c->depth_scaled_alt, P)); c->pf_built = false; c->frontend_ready = false;
-    KT_TRY(dev_alloc(c, &c->ztable, (size_t)2 * cfg->vol)); KT_TRY(dev_alloc(c, &c->cw_scratch, P)); KT_TRY(dev_alloc(c, &c->rgbf_scratch, P * 4)); KT_TRY(dev_alloc(c, &c->cw_alt, P)); KT_TRY(dev_alloc(c, &c->rgbf_alt, P * 4));
+    c->vmap_curr_color = c->arena + c->off_vcol; if (dev(&c->depth_scaled, P) || dev(&c->depth_scaled_alt, P)) return KT_ERR_CUDA; c->pf_built = false; c->frontend_ready = false;
+    if (dev(&c->ztable, (size_t)2 * cfg->vol) || dev(&c->cw_scratch, P) || dev(&c->rgbf_scratch, P * 4) || dev(&c->cw_alt, P) || dev(&c->rgbf_alt, P * 4)) return KT_ERR_CUDA;
 
-    KT_TRY(dev_alloc(c, &c->state, 1)); KT_TRY(dev_alloc(c, &c->partials, (size_t)MAX_PARTIALS * 32));
-    KT_TRY(kt::cuda_check(cudaMemset(c->partials, 0, (size_t)MAX_PARTIALS * 32 * sizeof(float)), "memset", __FILE__, __LINE__));   // tags start at 0
-    KT_TRY(dev_alloc(c, &c->prof_dev, 64 * 8)); KT_TRY(dev_alloc(c, &c->ipartials, (size_t)MAX_PARTIALS * 2));
-    KT_TRY(dev_alloc(c, &c->trace_dev, (size_t)MAX_TRACE_ITERS * TRACE_STRIDE)); KT_TRY(dev_alloc(c, &c->pose12_dev, 12));
+    if (dev(&c->state, 1) || dev(&c->partials, (size_t)MAX_PARTIALS * 32)) return KT_ERR_CUDA;
+    KT_CUDA(cudaMemset(c->partials, 0, (size_t)MAX_PARTIALS * 32 * sizeof(float)));   // tags start at 0
+    if (dev(&c->prof_dev, 64 * 8) || dev(&c->ipartials, (size_t)MAX_PARTIALS * 2)) return KT_ERR_CUDA;
+    if (dev(&c->trace_dev, (size_t)MAX_TRACE_ITERS * TRACE_STRIDE) || dev(&c->pose12_dev, 12)) return KT_ERR_CUDA;
     c->cloud_capacity = (size_t)c->cfg.cloud_capacity;
-    KT_TRY(dev_alloc(c, &c->cloud_dev, c->cloud_capacity)); KT_TRY(dev_alloc(c, &c->counter_dev, 1));
-    c->slice_arena = new PinnedArena();
+    if (dev(&c->cloud_dev, c->cloud_capacity) || dev(&c->counter_dev, 1)) return KT_ERR_CUDA;
     c->mesh_weight_cull = 8;                                   // -cw default, also the live mesh's until kt_set_slice_meshing
-    if (!c->slice_arena->alloc(256)) { set_error("kt_create: pinned slice arena"); kt_destroy(c); return KT_ERR_CUDA; }      // the first 64 MB slab now, not inside the first shift frame
-    c->slice_arena->rewind();
-    KT_TRY(kt::cuda_check(cudaStreamCreateWithFlags(&c->stream_slices, cudaStreamNonBlocking), "stream_slices", __FILE__, __LINE__));
-    KT_TRY(kt::cuda_check(cudaEventCreateWithFlags(&c->ev_cloud_ready, cudaEventDisableTiming), "event", __FILE__, __LINE__));
-    KT_TRY(kt::cuda_check(cudaEventCreateWithFlags(&c->ev_cloud_free, cudaEventDisableTiming), "event", __FILE__, __LINE__));
-    KT_TRY(kt::cuda_check(cudaMallocHost((void**)&c->pose12_host, 12 * sizeof(float)), "pinned", __FILE__, __LINE__));
-    KT_TRY(kt::cuda_check(cudaHostAlloc((void**)&c->result_host, sizeof(OdomResult), cudaHostAllocMapped), "pinned", __FILE__, __LINE__));
+    if (!c->slice_arena.alloc(256)) return KT_ERR_CUDA;      // the first 64 MB slab now, not inside the first shift frame
+    c->slice_arena.rewind();
+    if (c->mem.stream(&c->stream_slices, W)) return KT_ERR_CUDA;
+    if (event(&c->ev_cloud_ready, cudaEventDisableTiming)) return KT_ERR_CUDA;
+    if (event(&c->ev_cloud_free, cudaEventDisableTiming)) return KT_ERR_CUDA;
+    if (c->mem.pinned(&c->pose12_host, 12, W)) return KT_ERR_CUDA;
+    if (c->mem.mapped(&c->result_host, 1, W)) return KT_ERR_CUDA;
     std::memset(c->result_host, 0, sizeof(OdomResult));
-    { void* dp = 0; KT_TRY(kt::cuda_check(cudaHostGetDevicePointer(&dp, c->result_host, 0), "mapped", __FILE__, __LINE__)); c->result_dev_alias = (float*)dp; }
+    { void* dp = 0; KT_CUDA(cudaHostGetDevicePointer(&dp, c->result_host, 0)); c->result_dev_alias = (float*)dp; }
     c->pose_seq = 0;
-    KT_TRY(kt::cuda_check(cudaMallocHost((void**)&c->trace_host, (size_t)MAX_TRACE_ITERS * TRACE_STRIDE * sizeof(float)), "pinned", __FILE__, __LINE__));
-    KT_TRY(kt::cuda_check(cudaMallocHost((void**)&c->counter_host, sizeof(unsigned int)), "pinned", __FILE__, __LINE__));
-    for (int i = 0; i < 7; ++i) KT_TRY(kt::cuda_check(cudaEventCreate(&c->ev[i]), "event", __FILE__, __LINE__));
-    for (int i = 0; i < 2; ++i) KT_TRY(kt::cuda_check(cudaEventCreate(&c->ev_icp[i]), "event", __FILE__, __LINE__));
-    for (int i = 0; i < 4; ++i) KT_TRY(kt::cuda_check(cudaEventCreate(&c->ev_krn[i]), "event", __FILE__, __LINE__));
-    for (int i = 0; i < 2; ++i) KT_TRY(kt::cuda_check(cudaEventCreate(&c->ev_span[i]), "event", __FILE__, __LINE__));
+    if (c->mem.pinned(&c->trace_host, (size_t)MAX_TRACE_ITERS * TRACE_STRIDE, W)) return KT_ERR_CUDA;
+    if (c->mem.pinned(&c->counter_host, 1, W)) return KT_ERR_CUDA;
+    for (int i = 0; i < 7; ++i) if (event(&c->ev[i], cudaEventDefault)) return KT_ERR_CUDA;
+    for (int i = 0; i < 2; ++i) if (event(&c->ev_icp[i], cudaEventDefault)) return KT_ERR_CUDA;
+    for (int i = 0; i < 4; ++i) if (event(&c->ev_krn[i], cudaEventDefault)) return KT_ERR_CUDA;
+    for (int i = 0; i < 2; ++i) if (event(&c->ev_span[i], cudaEventDefault)) return KT_ERR_CUDA;
     for (int i = 0; i < 6; ++i) c->stage_ms[i] = 0.f;
-    KT_TRY(kt_reset(c));
-#undef KT_TRY
-    *out = c;
+    int r = kt_reset(c); if (r) return r;
+    *out = owner.release();
     return KT_OK;
 }
 
 int kt_destroy(kt_ctx* c)
 {
-    if (!c) return KT_OK;
-    cudaSetDevice(c->cfg.device);
-    if (c->stream) cudaStreamSynchronize(c->stream);
-    for (int g = 0; g < MAX_GPUS; ++g) if (c->peer_arena[g] && c->peer_arena[g] != c->arena) cudaIpcCloseMemHandle(c->peer_arena[g]);
-    if (c->mg_error_host) cudaFreeHost(c->mg_error_host);
-    place_free(c->place); c->place = 0;
-    drop_slices(c);
-    if (c->pose_log) fclose(c->pose_log);
-    if (c->slice_arena) { c->slice_arena->release(); delete c->slice_arena; }
-    if (c->deform_arena) { c->deform_arena->release(); delete c->deform_arena; }
-    slice_ws_free(&c->slice_ws);
-    mesh_ws_free(&c->mesh_ws);
-    if (c->mesh_verts_dev) cudaFree(c->mesh_verts_dev);
-    if (c->mesh_tris_dev) cudaFree(c->mesh_tris_dev);
-    if (c->stream_slices) cudaStreamDestroy(c->stream_slices);
-    if (c->ev_cloud_ready) cudaEventDestroy(c->ev_cloud_ready);
-    if (c->ev_cloud_free) cudaEventDestroy(c->ev_cloud_free);
-    for (void* p : c->allocs) cudaFree(p);
-    if (c->pose12_host) cudaFreeHost(c->pose12_host);
-    if (c->result_host) cudaFreeHost(c->result_host);
-    if (c->trace_host) cudaFreeHost(c->trace_host);
-    if (c->counter_host) cudaFreeHost(c->counter_host);
-    for (int i = 0; i < 7; ++i) if (c->ev[i]) cudaEventDestroy(c->ev[i]);
-    for (int i = 0; i < 2; ++i) if (c->ev_icp[i]) cudaEventDestroy(c->ev_icp[i]);
-    for (int i = 0; i < 4; ++i) if (c->ev_krn[i]) cudaEventDestroy(c->ev_krn[i]);
-    for (int i = 0; i < 2; ++i) if (c->ev_span[i]) cudaEventDestroy(c->ev_span[i]);
-    if (c->stream_copy) { cudaStreamSynchronize(c->stream_copy); cudaStreamDestroy(c->stream_copy); }
-    if (c->ev_prefetch) cudaEventDestroy(c->ev_prefetch);
-    if (c->ev_maps) cudaEventDestroy(c->ev_maps);
-    for (int i = 0; i < 2; ++i) if (c->ev_done[i]) cudaEventDestroy(c->ev_done[i]);
-    if (c->stream) cudaStreamDestroy(c->stream);
     delete c;
     return KT_OK;
 }
@@ -1041,7 +982,7 @@ int kt_get_slice(kt_ctx* c, int idx, kt_point_xyzrgb* points, size_t max_points,
     if (camera_t) for (int i = 0; i < 3; ++i) camera_t[i] = s.camera_t[i];
     size_t n = std::min(max_points, s.count);
     if (points && n) {
-        KT_CUDA(cudaEventSynchronize(s.ready));                  // the asynchronous download of this slice has landed
+        KT_CUDA(cudaEventSynchronize(s.ready.get()));                  // the asynchronous download of this slice has landed
         std::memcpy(points, s.points, n * sizeof(kt_point_xyzrgb));
     }
     return KT_OK;
@@ -1085,7 +1026,7 @@ int kt_get_processed_slice(kt_ctx* c, int idx, kt_point_xyzrgbnormal* points, si
     if (count) *count = s.processed_count;
     size_t n = std::min(max_points, s.processed_count);
     if (points && n) {
-        KT_CUDA(cudaEventSynchronize(s.ready));
+        KT_CUDA(cudaEventSynchronize(s.ready.get()));
         std::memcpy(points, s.processed, n * sizeof(kt_point_xyzrgbnormal));
     }
     return KT_OK;
@@ -1107,7 +1048,7 @@ int kt_get_slice_mesh(kt_ctx* c, int idx, kt_mesh_vertex* verts, size_t max_vert
     if (n_verts) *n_verts = s.mesh_nv;
     if (n_tris) *n_tris = s.mesh_nt;
     const size_t nv = verts ? std::min(max_verts, s.mesh_nv) : 0, nt = tris ? std::min(max_tris, s.mesh_nt) : 0;
-    if (nv || nt) KT_CUDA(cudaEventSynchronize(s.ready));
+    if (nv || nt) KT_CUDA(cudaEventSynchronize(s.ready.get()));
     if (nv) std::memcpy(verts, s.mesh_verts, nv * sizeof(kt_mesh_vertex));
     if (nt) std::memcpy(tris, s.mesh_tris, nt * 3 * sizeof(uint32_t));
     return KT_OK;
@@ -1126,8 +1067,8 @@ int kt_get_live_mesh(kt_ctx* c, kt_mesh_vertex* verts, size_t max_verts, uint32_
     if (n_verts) *n_verts = c->mesh_nv;
     if (n_tris) *n_tris = c->mesh_nt;
     const size_t nv = verts ? std::min(max_verts, c->mesh_nv) : 0, nt = tris ? std::min(max_tris, c->mesh_nt) : 0;
-    if (nv) KT_CUDA(cudaMemcpyAsync(verts, c->mesh_verts_dev, nv * sizeof(kt_mesh_vertex), cudaMemcpyDeviceToHost, c->stream));
-    if (nt) KT_CUDA(cudaMemcpyAsync(tris, c->mesh_tris_dev, nt * 3 * sizeof(uint32_t), cudaMemcpyDeviceToHost, c->stream));
+    if (nv) KT_CUDA(cudaMemcpyAsync(verts, c->mesh_verts.get(), nv * sizeof(kt_mesh_vertex), cudaMemcpyDeviceToHost, c->stream));
+    if (nt) KT_CUDA(cudaMemcpyAsync(tris, c->mesh_tris.get(), nt * 3 * sizeof(uint32_t), cudaMemcpyDeviceToHost, c->stream));
     KT_CUDA(cudaStreamSynchronize(c->stream));
     return KT_OK;
 }
@@ -1149,7 +1090,7 @@ static int save_mesh_ply(kt_ctx* c, const char* path, size_t n_slices, bool defo
     for (size_t k = 0; k < n_slices; ++k) {                        // x86 / aarch64 hosts are little-endian: records are the raw bytes
         const auto& s = c->slices[k];
         if (!s.has_mesh || !s.mesh_nv) continue;
-        if (cudaEventSynchronize(s.ready) != cudaSuccess) { ok = false; break; }
+        if (cudaEventSynchronize(s.ready.get()) != cudaSuccess) { ok = false; break; }
         const kt_mesh_vertex* mv = deformed ? c->deformed[k].mesh_verts : s.mesh_verts;
         buf.resize(s.mesh_nv * 27);
         for (size_t i = 0; i < s.mesh_nv; ++i) {
@@ -1223,70 +1164,60 @@ static int deform_run(kt_ctx* c, const std::vector<float>& npos, const std::vect
     KT_CUDA(cudaSetDevice(c->cfg.device));
     if (c->stream_slices) KT_CUDA(cudaStreamSynchronize(c->stream_slices));           // every slice has landed in its pinned buffers
     const size_t nmax = std::max(std::max(np, nm), m);
-    float* d_npos = 0; uint64_t* d_ntime = 0; double* d_x = 0; uint64_t* d_t = 0; int32_t* d_ids = 0; double* d_w = 0; void* d_in = 0; void* d_out = 0;
-    auto cleanup = [&]() { cudaFree(d_npos); cudaFree(d_ntime); cudaFree(d_x); cudaFree(d_t); cudaFree(d_ids); cudaFree(d_w); cudaFree(d_in); cudaFree(d_out); };
-    auto run = [&]() -> int {
-        cudaStream_t s = c->stream;
-        KT_CUDA(cudaMalloc((void**)&d_npos, npos.size() * sizeof(float)));
-        KT_CUDA(cudaMalloc((void**)&d_ntime, ntime.size() * sizeof(uint64_t)));
-        KT_CUDA(cudaMalloc((void**)&d_x, (size_t)nn * 12 * sizeof(double)));
-        KT_CUDA(cudaMalloc((void**)&d_t, nmax * sizeof(uint64_t)));
-        KT_CUDA(cudaMalloc((void**)&d_ids, nmax * 4 * sizeof(int32_t)));
-        KT_CUDA(cudaMalloc((void**)&d_w, nmax * 4 * sizeof(double)));
-        KT_CUDA(cudaMalloc(&d_in, nmax * sizeof(kt_point_xyzrgbnormal)));
-        KT_CUDA(cudaMemcpyAsync(d_npos, npos.data(), npos.size() * sizeof(float), cudaMemcpyHostToDevice, s));
-        KT_CUDA(cudaMemcpyAsync(d_ntime, ntime.data(), ntime.size() * sizeof(uint64_t), cudaMemcpyHostToDevice, s));
-        // constraint weights (their sources are vertices of the graph too: appendVertices) -> optimiseGraphSparse
-        KT_CUDA(cudaMemcpyAsync(d_in, csrc.data(), csrc.size() * sizeof(float), cudaMemcpyHostToDevice, s));
-        KT_CUDA(cudaMemcpyAsync(d_t, ct.data(), m * sizeof(uint64_t), cudaMemcpyHostToDevice, s));
-        int r = deform_weights(d_npos, d_ntime, nn, d_in, 2, d_t, m, d_ids, d_w, s); if (r) return r;
-        std::vector<int32_t> cids(4 * m); std::vector<double> cw(4 * m);
-        KT_CUDA(cudaMemcpyAsync(cids.data(), d_ids, cids.size() * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
-        KT_CUDA(cudaMemcpyAsync(cw.data(), d_w, cw.size() * sizeof(double), cudaMemcpyDeviceToHost, s));
-        KT_CUDA(cudaStreamSynchronize(s));
-        r = deform_optimise(npos.data(), nn, csrc.data(), cdst.data(), cids.data(), cw.data(), m, d_x, report, s); if (r) return r;
-        c->deformed.assign(c->slices.size(), kt_ctx::Deformed());
-        for (size_t i = 0; i < c->slices.size(); ++i) { c->deformed[i].processed = c->slices[i].processed; c->deformed[i].mesh_verts = c->slices[i].mesh_verts; }
-        if (!report->deformed) return 0;                                                  // the map as recorded
-        if (!c->deform_arena) c->deform_arena = new PinnedArena();
-        c->deform_arena->rewind();
-        KT_CUDA(cudaMalloc(&d_out, nmax * sizeof(kt_point_xyzrgbnormal)));
-        // the map, one kind at a time: upload from the slices' pinned buffers, weights, apply, download into the deformation arena
-        for (int kind = 0; kind < 2; ++kind) {
-            const size_t total = kind == 0 ? np : nm, rec = kind == 0 ? sizeof(kt_point_xyzrgbnormal) : sizeof(kt_mesh_vertex);
-            if (!total) continue;
-            std::vector<uint64_t> vt(total);
-            size_t off = 0;
-            for (const auto& sl : c->slices) {
-                const size_t cnt = kind == 0 ? (sl.has_processed ? sl.processed_count : 0) : (sl.has_mesh ? sl.mesh_nv : 0);
-                if (!cnt) continue;
-                KT_CUDA(cudaMemcpyAsync((char*)d_in + off * rec, kind == 0 ? (const void*)sl.processed : (const void*)sl.mesh_verts, cnt * rec, cudaMemcpyHostToDevice, s));
-                std::fill(vt.begin() + off, vt.begin() + off + cnt, sl.utime);             // a vertex's time is its slice's
-                off += cnt;
-            }
-            KT_CUDA(cudaMemcpyAsync(d_t, vt.data(), total * sizeof(uint64_t), cudaMemcpyHostToDevice, s));
-            r = deform_weights(d_npos, d_ntime, nn, d_in, kind, d_t, total, d_ids, d_w, s); if (r) return r;
-            r = deform_apply(d_npos, d_x, nn, d_ids, d_w, d_in, d_out, kind, total, s); if (r) return r;
-            off = 0;
-            for (size_t i = 0; i < c->slices.size(); ++i) {
-                const auto& sl = c->slices[i];
-                const size_t cnt = kind == 0 ? (sl.has_processed ? sl.processed_count : 0) : (sl.has_mesh ? sl.mesh_nv : 0);
-                if (!cnt) continue;
-                void* h = c->deform_arena->alloc(cnt * rec);
-                if (!h) { set_error("kt_deform_map: pinned host memory for %zu deformed records", cnt); return KT_ERR_CUDA; }
-                KT_CUDA(cudaMemcpyAsync(h, (const char*)d_out + off * rec, cnt * rec, cudaMemcpyDeviceToHost, s));
-                if (kind == 0) c->deformed[i].processed = (kt_point_xyzrgbnormal*)h; else c->deformed[i].mesh_verts = (kt_mesh_vertex*)h;
-                off += cnt;
-            }
-            KT_CUDA(cudaStreamSynchronize(s));                                            // vt and the device buffers are reused
+    // the scratch below is freed after the tracker stream has finished with it; c->deformed is left empty on an error
+    c->deformed.clear();
+    cudaStream_t s = c->stream;
+    Allocations mem(s); const char* W = "kt_deform_map scratch";
+    float* d_npos; uint64_t* d_ntime; double* d_x; uint64_t* d_t; int32_t* d_ids; double* d_w; unsigned char* d_in; unsigned char* d_out;
+    if (mem.device(&d_npos, npos.size(), W) || mem.device(&d_ntime, ntime.size(), W) || mem.device(&d_x, (size_t)nn * 12, W) ||
+        mem.device(&d_t, nmax, W) || mem.device(&d_ids, nmax * 4, W) || mem.device(&d_w, nmax * 4, W) || mem.device(&d_in, nmax * sizeof(kt_point_xyzrgbnormal), W)) return KT_ERR_CUDA;
+    KT_CUDA(cudaMemcpyAsync(d_npos, npos.data(), npos.size() * sizeof(float), cudaMemcpyHostToDevice, s));
+    KT_CUDA(cudaMemcpyAsync(d_ntime, ntime.data(), ntime.size() * sizeof(uint64_t), cudaMemcpyHostToDevice, s));
+    // constraint weights (their sources are vertices of the graph too: appendVertices) -> optimiseGraphSparse
+    KT_CUDA(cudaMemcpyAsync(d_in, csrc.data(), csrc.size() * sizeof(float), cudaMemcpyHostToDevice, s));
+    KT_CUDA(cudaMemcpyAsync(d_t, ct.data(), m * sizeof(uint64_t), cudaMemcpyHostToDevice, s));
+    int r = deform_weights(d_npos, d_ntime, nn, d_in, 2, d_t, m, d_ids, d_w, s); if (r) return r;
+    std::vector<int32_t> cids(4 * m); std::vector<double> cw(4 * m);
+    KT_CUDA(cudaMemcpyAsync(cids.data(), d_ids, cids.size() * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
+    KT_CUDA(cudaMemcpyAsync(cw.data(), d_w, cw.size() * sizeof(double), cudaMemcpyDeviceToHost, s));
+    KT_CUDA(cudaStreamSynchronize(s));
+    r = deform_optimise(npos.data(), nn, csrc.data(), cdst.data(), cids.data(), cw.data(), m, d_x, report, s); if (r) return r;
+    std::vector<kt_ctx::Deformed> def(c->slices.size());
+    for (size_t i = 0; i < c->slices.size(); ++i) { def[i].processed = c->slices[i].processed; def[i].mesh_verts = c->slices[i].mesh_verts; }
+    if (!report->deformed) { c->deformed = std::move(def); return 0; }               // the map as recorded
+    c->deform_arena.rewind();
+    if (mem.device(&d_out, nmax * sizeof(kt_point_xyzrgbnormal), W)) return KT_ERR_CUDA;
+    // the map, one kind at a time: upload from the slices' pinned buffers, weights, apply, download into the deformation arena
+    for (int kind = 0; kind < 2; ++kind) {
+        const size_t total = kind == 0 ? np : nm, rec = kind == 0 ? sizeof(kt_point_xyzrgbnormal) : sizeof(kt_mesh_vertex);
+        if (!total) continue;
+        std::vector<uint64_t> vt(total);
+        size_t off = 0;
+        for (const auto& sl : c->slices) {
+            const size_t cnt = kind == 0 ? (sl.has_processed ? sl.processed_count : 0) : (sl.has_mesh ? sl.mesh_nv : 0);
+            if (!cnt) continue;
+            KT_CUDA(cudaMemcpyAsync((char*)d_in + off * rec, kind == 0 ? (const void*)sl.processed : (const void*)sl.mesh_verts, cnt * rec, cudaMemcpyHostToDevice, s));
+            std::fill(vt.begin() + off, vt.begin() + off + cnt, sl.utime);             // a vertex's time is its slice's
+            off += cnt;
         }
-        return 0;
-    };
-    const int r = run();
-    cudaStreamSynchronize(c->stream);
-    cleanup();
-    if (r) c->deformed.clear();
-    return r;
+        KT_CUDA(cudaMemcpyAsync(d_t, vt.data(), total * sizeof(uint64_t), cudaMemcpyHostToDevice, s));
+        r = deform_weights(d_npos, d_ntime, nn, d_in, kind, d_t, total, d_ids, d_w, s); if (r) return r;
+        r = deform_apply(d_npos, d_x, nn, d_ids, d_w, d_in, d_out, kind, total, s); if (r) return r;
+        off = 0;
+        for (size_t i = 0; i < c->slices.size(); ++i) {
+            const auto& sl = c->slices[i];
+            const size_t cnt = kind == 0 ? (sl.has_processed ? sl.processed_count : 0) : (sl.has_mesh ? sl.mesh_nv : 0);
+            if (!cnt) continue;
+            void* h = c->deform_arena.alloc(cnt * rec);
+            if (!h) { set_error("kt_deform_map: pinned host memory for %zu deformed records", cnt); return KT_ERR_CUDA; }
+            KT_CUDA(cudaMemcpyAsync(h, (const char*)d_out + off * rec, cnt * rec, cudaMemcpyDeviceToHost, s));
+            if (kind == 0) def[i].processed = (kt_point_xyzrgbnormal*)h; else def[i].mesh_verts = (kt_mesh_vertex*)h;
+            off += cnt;
+        }
+        KT_CUDA(cudaStreamSynchronize(s));                                            // vt and the device buffers are reused
+    }
+    c->deformed = std::move(def);
+    return 0;
 }
 
 
@@ -1392,16 +1323,17 @@ int kt_close_loop(kt_ctx* c, const kt_loop_constraint* loop, float pose_spacing,
     }
 
     KT_CUDA(cudaSetDevice(c->cfg.device));
-    double* d_X = 0;
-    KT_CUDA(cudaMalloc((void**)&d_X, X0.size() * sizeof(double)));
     std::vector<double> X(X0.size());
     kt_pgo_report pr;
-    int r = 0;
-    if (!(r = kt::cuda_check(cudaMemcpyAsync(d_X, X0.data(), X0.size() * sizeof(double), cudaMemcpyHostToDevice, c->stream), "upload", __FILE__, __LINE__)))
-        r = pgo_optimise(d_X, n, f.data(), (int)f.size(), d_X, &pr, c->stream);
-    if (!r) r = kt::cuda_check(cudaMemcpy(X.data(), d_X, X.size() * sizeof(double), cudaMemcpyDeviceToHost), "download", __FILE__, __LINE__);
-    cudaFree(d_X);
-    if (r) return r;
+    int r;
+    {   // the poses on the device, freed after the tracker stream has finished with them
+        Allocations mem(c->stream);
+        double* d_X;
+        if ((r = mem.device(&d_X, X0.size(), "kt_close_loop poses"))) return r;
+        KT_CUDA(cudaMemcpyAsync(d_X, X0.data(), X0.size() * sizeof(double), cudaMemcpyHostToDevice, c->stream));
+        if ((r = pgo_optimise(d_X, n, f.data(), (int)f.size(), d_X, &pr, c->stream))) return r;
+        KT_CUDA(cudaMemcpy(X.data(), d_X, X.size() * sizeof(double), cudaMemcpyDeviceToHost));
+    }
     report->nodes = pr.nodes; report->factors = pr.factors; report->loops = pr.loops; report->iterations = pr.iterations;
     report->chi2_initial = pr.chi2_initial; report->chi2_final = pr.chi2_final; report->solver_failed = pr.solver_failed;
     report->accepted = !pr.solver_failed && pr.chi2_final < isam_thresh;          // Deformation.cpp:256
@@ -1467,44 +1399,38 @@ int kt_set_loop_detection(kt_ctx* c, const kt_loop_detection_params* p)
 {
     if (!c) return KT_ERR_INVALID;
     KT_CUDA(cudaSetDevice(c->cfg.device));
-    if (!p || !p->enabled) { place_free(c->place); c->place = 0; return KT_OK; }
+    if (!p || !p->enabled) { c->place.reset(); return KT_OK; }
     if (c->world > 1) { set_error("kt_set_loop_detection: a volume shared by %d GPUs has no loop detection", c->world); return KT_ERR_INVALID; }
     if (p->max_keyframes < 1 || p->max_features < 2 || p->exclude_recent < 1 || !(p->inlier_ratio >= 0.f) || !(p->loop_throttle_s >= 0.0)) {
         set_error("kt_set_loop_detection: bad parameters"); return KT_ERR_INVALID;
     }
     if (c->place) {          // new parameters; the store is kept when its shape is unchanged
         if (c->place->maxK == p->max_keyframes && c->place->maxF == p->max_features) { c->place->p = *p; return KT_OK; }
-        place_free(c->place); c->place = 0;
+        c->place.reset();
     }
-    PlaceStore* ps = new PlaceStore();
+    std::unique_ptr<PlaceStore> ps(new PlaceStore());
     ps->p = *p; ps->rows = c->cfg.rows; ps->cols = c->cfg.cols; ps->maxK = p->max_keyframes; ps->maxF = p->max_features;
     const size_t P = (size_t)ps->rows * ps->cols, K = (size_t)ps->maxK, F = (size_t)ps->maxF;
-    int r = 0;
-#define PS_TRY(x) do { if ((r = (x))) { place_free(ps); return r; } } while (0)
-    PS_TRY(cuda_check(cudaStreamCreateWithFlags(&ps->stream, cudaStreamNonBlocking), "stream", __FILE__, __LINE__));
-    PS_TRY(cuda_check(cudaEventCreateWithFlags(&ps->ev_input, cudaEventDisableTiming), "event", __FILE__, __LINE__));
-    PS_TRY(cuda_check(cudaEventCreateWithFlags(&ps->ev_copied, cudaEventDisableTiming), "event", __FILE__, __LINE__));
-    PS_TRY(cuda_check(cudaMallocHost((void**)&ps->nfeat_host, K * sizeof(int)), "pinned", __FILE__, __LINE__));
-    PS_TRY(ps->alloc(&ps->depth, K * P)); PS_TRY(ps->alloc(&ps->rgb, P * 3)); PS_TRY(ps->alloc(&ps->kp, K * F * 6)); PS_TRY(ps->alloc(&ps->desc, K * F * 64));
-    PS_TRY(ps->alloc(&ps->xyz, K * F * 3)); PS_TRY(ps->alloc(&ps->nfeat_dev, K));
-    PS_TRY(ps->alloc(&ps->best, K * F)); PS_TRY(ps->alloc(&ps->d1, K * F)); PS_TRY(ps->alloc(&ps->d2, K * F)); PS_TRY(ps->alloc(&ps->pass, K * F));
-    PS_TRY(ps->alloc(&ps->seg_passes, K));
-    PS_TRY(ps->alloc(&ps->pn, F * 3)); PS_TRY(ps->alloc(&ps->po, F * 3)); PS_TRY(ps->alloc(&ps->uv, F * 2)); PS_TRY(ps->alloc(&ps->pose, 12));
-    PS_TRY(ps->alloc(&ps->inl, F)); PS_TRY(ps->alloc(&ps->ninl, 1));
+    const char* W = "the loop detection store";
+    auto dev = [&](auto** q, size_t n) { return ps->mem.device(q, n, W); };
+    if (ps->mem.stream(&ps->stream, W) || ps->mem.event(&ps->ev_input, cudaEventDisableTiming, W) || ps->mem.event(&ps->ev_copied, cudaEventDisableTiming, W) ||
+        ps->mem.pinned(&ps->nfeat_host, K, W)) return KT_ERR_CUDA;
+    if (dev(&ps->depth, K * P) || dev(&ps->rgb, P * 3) || dev(&ps->kp, K * F * 6) || dev(&ps->desc, K * F * 64) || dev(&ps->xyz, K * F * 3) || dev(&ps->nfeat_dev, K) ||
+        dev(&ps->best, K * F) || dev(&ps->d1, K * F) || dev(&ps->d2, K * F) || dev(&ps->pass, K * F) || dev(&ps->seg_passes, K) ||
+        dev(&ps->pn, F * 3) || dev(&ps->po, F * 3) || dev(&ps->uv, F * 2) || dev(&ps->pose, 12) || dev(&ps->inl, F) || dev(&ps->ninl, 1)) return KT_ERR_CUDA;
     for (int s2 = 0; s2 < 2; ++s2) {
         for (int l = 0; l < LEVELS; ++l) {
             const size_t Pl = P >> (2 * l);
-            PS_TRY(ps->alloc(&ps->depths[s2][l], Pl)); PS_TRY(ps->alloc(&ps->vmaps[s2][l], Pl * 3)); PS_TRY(ps->alloc(&ps->nmaps[s2][l], Pl * 3));
-            PS_TRY(cuda_check(cudaMemset(ps->vmaps[s2][l], 0, Pl * 12), "memset", __FILE__, __LINE__));
-            PS_TRY(cuda_check(cudaMemset(ps->nmaps[s2][l], 0, Pl * 12), "memset", __FILE__, __LINE__));
+            if (dev(&ps->depths[s2][l], Pl) || dev(&ps->vmaps[s2][l], Pl * 3) || dev(&ps->nmaps[s2][l], Pl * 3)) return KT_ERR_CUDA;
+            KT_CUDA(cudaMemset(ps->vmaps[s2][l], 0, Pl * 12));
+            KT_CUDA(cudaMemset(ps->nmaps[s2][l], 0, Pl * 12));
         }
-        PS_TRY(ps->alloc(&ps->cloud[s2], P)); PS_TRY(ps->alloc(&ps->cent[s2], P));
+        if (dev(&ps->cloud[s2], P) || dev(&ps->cent[s2], P)) return KT_ERR_CUDA;
     }
-    PS_TRY(ps->alloc(&ps->d2fit, P + 8));
-    PS_TRY(ps->alloc(&ps->state, 1)); PS_TRY(cuda_check(cudaMemset(ps->state, 0, sizeof(OdomState)), "memset", __FILE__, __LINE__));
-    PS_TRY(ps->alloc(&ps->xwords, odom_exchange_words())); PS_TRY(ps->alloc(&ps->trace, (size_t)MAX_TRACE_ITERS * TRACE_STRIDE));
-#undef PS_TRY
-    c->place = ps;
+    if (dev(&ps->d2fit, P + 8) || dev(&ps->state, 1)) return KT_ERR_CUDA;
+    KT_CUDA(cudaMemset(ps->state, 0, sizeof(OdomState)));
+    if (dev(&ps->xwords, odom_exchange_words()) || dev(&ps->trace, (size_t)MAX_TRACE_ITERS * TRACE_STRIDE)) return KT_ERR_CUDA;
+    c->place = std::move(ps);
     return KT_OK;
 }
 
@@ -1540,7 +1466,7 @@ void m4_rigid_inverse(const double* T, double* I)
 // One keyframe through the chain (PlaceRecognition::process + processLoopClosureDetection, PlaceRecognition.cpp:51-209).
 int place_process(kt_ctx* c, int q, kt_place_result* res)
 {
-    PlaceStore* ps = c->place;
+    PlaceStore* ps = c->place.get();
     cudaStream_t s = c->stream;
     const size_t P = (size_t)ps->rows * ps->cols, F = (size_t)ps->maxF;
     const float intr[4] = {c->cfg.fx, c->cfg.fy, c->cfg.cx, c->cfg.cy};
@@ -1672,7 +1598,7 @@ int kt_detect_loops(kt_ctx* c, kt_place_result* out, size_t capacity, size_t* n_
     if (c->world > 1) { set_error("kt_detect_loops: a volume shared by %d GPUs has no loop detection", c->world); return KT_ERR_INVALID; }
     if (!c->place) { set_error("kt_detect_loops: loop detection is off (kt_set_loop_detection)"); return KT_ERR_STATE; }
     KT_CUDA(cudaSetDevice(c->cfg.device));
-    PlaceStore* ps = c->place;
+    PlaceStore* ps = c->place.get();
     KT_CUDA(cudaStreamSynchronize(ps->stream));                  // every capture has landed
     ps->in_new.clear(); ps->in_old.clear();
     const size_t pending = ps->times.size() - ps->processed;
@@ -1775,64 +1701,54 @@ static int map_cloud(kt_ctx* c, int which, int dedupe, kt_point_xyzrgbnormal* ou
         }
     } else if (n) {
         cudaStream_t s = c->stream_slices;
-        void* d_in = 0; void* d_out = 0;
-        cudaEvent_t ev[4] = {0, 0, 0, 0};
-        auto run = [&]() -> int {
-            for (int e = 0; e < 4; ++e) KT_CUDA(cudaEventCreate(&ev[e]));
-            if (cudaMalloc(&d_in, n * rec) != cudaSuccess || (dedupe && cudaMalloc(&d_out, n * rec) != cudaSuccess)) {
-                cudaGetLastError();                                                    // not sticky: the next frame must not see it
-                set_error("%s: cannot allocate device memory for %zu points", who, n); return KT_ERR_CUDA;
-            }
-            KT_CUDA(cudaEventRecord(ev[0], s));
-            size_t off = 0;
-            for (size_t i = 0; i < c->slices.size(); ++i) {
-                const SliceRec& sl = c->slices[i];
-                if (!sl.has_processed || !sl.processed_count) continue;
-                KT_CUDA(cudaMemcpyAsync((char*)d_in + off * rec, src(i), sl.processed_count * rec, cudaMemcpyHostToDevice, s));
-                off += sl.processed_count;
-            }
-            KT_CUDA(cudaEventRecord(ev[1], s));
-            if (n_fixed < n) {
-                // C = P_corr(t) P_tracked(t)^-1 in FP64, the rigid inverse [R^T | -R^T t], rounded to float
-                const float* Pt = c->map_corr.tracked; const float* Pc = c->map_corr.corrected;
-                RigidF C;
-                for (int a = 0; a < 3; ++a) {
-                    for (int b = 0; b < 3; ++b) {
-                        double v = 0;
-                        for (int k = 0; k < 3; ++k) v += (double)Pc[4 * a + k] * (double)Pt[4 * b + k];
-                        C.R[3 * a + b] = (float)v;
-                    }
-                    double t = Pc[4 * a + 3];
-                    for (int b = 0; b < 3; ++b) {
-                        double v = 0;
-                        for (int k = 0; k < 3; ++k) v += (double)Pc[4 * a + k] * (double)Pt[4 * b + k];
-                        t -= v * (double)Pt[4 * b + 3];
-                    }
-                    C.t[a] = (float)t;
+        Allocations mem(s);
+        unsigned char* d_in = 0; unsigned char* d_out = 0;
+        cudaEvent_t ev[4];
+        for (int e = 0; e < 4; ++e) if (mem.event(&ev[e], cudaEventDefault, who)) return KT_ERR_CUDA;
+        if (mem.device(&d_in, n * rec, who) || (dedupe && mem.device(&d_out, n * rec, who))) return KT_ERR_CUDA;
+        KT_CUDA(cudaEventRecord(ev[0], s));
+        size_t off = 0;
+        for (size_t i = 0; i < c->slices.size(); ++i) {
+            const SliceRec& sl = c->slices[i];
+            if (!sl.has_processed || !sl.processed_count) continue;
+            KT_CUDA(cudaMemcpyAsync((char*)d_in + off * rec, src(i), sl.processed_count * rec, cudaMemcpyHostToDevice, s));
+            off += sl.processed_count;
+        }
+        KT_CUDA(cudaEventRecord(ev[1], s));
+        if (n_fixed < n) {
+            // C = P_corr(t) P_tracked(t)^-1 in FP64, the rigid inverse [R^T | -R^T t], rounded to float
+            const float* Pt = c->map_corr.tracked; const float* Pc = c->map_corr.corrected;
+            RigidF C;
+            for (int a = 0; a < 3; ++a) {
+                for (int b = 0; b < 3; ++b) {
+                    double v = 0;
+                    for (int k = 0; k < 3; ++k) v += (double)Pc[4 * a + k] * (double)Pt[4 * b + k];
+                    C.R[3 * a + b] = (float)v;
                 }
-                int r = rigid_move((kt_point_xyzrgbnormal*)d_in + n_fixed, n - n_fixed, C, s); if (r) return r;
+                double t = Pc[4 * a + 3];
+                for (int b = 0; b < 3; ++b) {
+                    double v = 0;
+                    for (int k = 0; k < 3; ++k) v += (double)Pc[4 * a + k] * (double)Pt[4 * b + k];
+                    t -= v * (double)Pt[4 * b + 3];
+                }
+                C.t[a] = (float)t;
             }
-            size_t m = n;
-            float ms2[2] = {0.f, 0.f};
-            if (dedupe) { int r = voxel_grid(d_in, n, 1, c->voxel, d_out, n, &m, &R.pcl_would_skip, ms2, s); if (r) return r; }
-            R.output_points = m;
-            if (grow) { grow->resize(m); out = grow->data(); capacity = m; }
-            KT_CUDA(cudaEventRecord(ev[2], s));
-            const size_t k = out ? std::min(m, capacity) : 0;
-            if (k) KT_CUDA(cudaMemcpyAsync(out, dedupe ? d_out : d_in, k * rec, cudaMemcpyDeviceToHost, s));
-            KT_CUDA(cudaEventRecord(ev[3], s));
-            KT_CUDA(cudaStreamSynchronize(s));
-            KT_CUDA(cudaEventElapsedTime(&R.upload_ms, ev[0], ev[1]));
-            KT_CUDA(cudaEventElapsedTime(&R.download_ms, ev[2], ev[3]));
-            KT_CUDA(cudaEventElapsedTime(&R.total_ms, ev[0], ev[3]));
-            R.sort_ms = ms2[0]; R.centroid_ms = ms2[1];
-            return 0;
-        };
-        const int r = run();
-        cudaStreamSynchronize(s);
-        cudaFree(d_in); cudaFree(d_out);
-        for (int e = 0; e < 4; ++e) if (ev[e]) cudaEventDestroy(ev[e]);
-        if (r) return r;
+            int r = rigid_move((kt_point_xyzrgbnormal*)d_in + n_fixed, n - n_fixed, C, s); if (r) return r;
+        }
+        size_t m = n;
+        float ms2[2] = {0.f, 0.f};
+        if (dedupe) { int r = voxel_grid(d_in, n, 1, c->voxel, d_out, n, &m, &R.pcl_would_skip, ms2, s); if (r) return r; }
+        R.output_points = m;
+        if (grow) { grow->resize(m); out = grow->data(); capacity = m; }
+        KT_CUDA(cudaEventRecord(ev[2], s));
+        const size_t k = out ? std::min(m, capacity) : 0;
+        if (k) KT_CUDA(cudaMemcpyAsync(out, dedupe ? d_out : d_in, k * rec, cudaMemcpyDeviceToHost, s));
+        KT_CUDA(cudaEventRecord(ev[3], s));
+        KT_CUDA(cudaStreamSynchronize(s));
+        KT_CUDA(cudaEventElapsedTime(&R.upload_ms, ev[0], ev[1]));
+        KT_CUDA(cudaEventElapsedTime(&R.download_ms, ev[2], ev[3]));
+        KT_CUDA(cudaEventElapsedTime(&R.total_ms, ev[0], ev[3]));
+        R.sort_ms = ms2[0]; R.centroid_ms = ms2[1];
     }
     if (count) *count = R.output_points;
     if (report) *report = R;
@@ -2096,11 +2012,11 @@ int kt_get_live_image(kt_ctx* c, uint8_t* shaded_rgb_host, uint8_t* color_rgb_ho
     if (!c) return KT_ERR_INVALID;
     KT_CUDA(cudaSetDevice(c->cfg.device));
     const size_t P = (size_t)c->cfg.rows * c->cfg.cols;
-    if (!c->view_dev) { int r = dev_alloc(c, &c->view_dev, P * 8); if (r) return r; }
-    uint8_t* shaded = c->view_dev; uint8_t* col = c->view_dev + P * 3; uint16_t* dep = (uint16_t*)(c->view_dev + P * 6);
+    int r = c->view.grow(P * 8, P * 8, "kt_get_live_image"); if (r) return r;
+    uint8_t* shaded = c->view.get(); uint8_t* col = shaded + P * 3; uint16_t* dep = (uint16_t*)(shaded + P * 6);
     const float light[3] = {c->size * -3.f, c->size * -3.f, c->size * -3.f};
     const M3 Rinv = m3_inverse(c->rmats.back());
-    int r = generate_views(c->vmaps_g_prev[0], c->nmaps_g_prev[0], c->vmap_curr_color, c->cfg.rows, c->cfg.cols, light, 1,
+    r = generate_views(c->vmaps_g_prev[0], c->nmaps_g_prev[0], c->vmap_curr_color, c->cfg.rows, c->cfg.cols, light, 1,
                            shaded_rgb_host ? shaded : 0, color_rgb_host ? col : 0, Rinv.m, c->tvecs.back().v, model_depth_host ? dep : 0, c->stream);
     if (r) return r;
     if (shaded_rgb_host) KT_CUDA(cudaMemcpyAsync(shaded_rgb_host, shaded, P * 3, cudaMemcpyDeviceToHost, c->stream));
@@ -2136,7 +2052,7 @@ int kt_debug_last_integrate(kt_ctx* c, float* Rinv9, float* t3, int* wrap3)
 
 long long kt_launch_count(kt_ctx* c) { return c ? g_launches.load() - c->launches_at_create : g_launches.load(); }
 
-int kt_alloc_pinned(void** ptr, size_t bytes) { KT_CUDA(cudaMallocHost(ptr, bytes)); return KT_OK; }
-int kt_free_pinned(void* ptr) { if (ptr) KT_CUDA(cudaFreeHost(ptr)); return KT_OK; }
+int kt_alloc_pinned(void** ptr, size_t bytes) { return host_malloc(ptr, bytes, "kt_alloc_pinned"); }
+int kt_free_pinned(void* ptr) { if (ptr) KT_CUDA(host_free(ptr)); return KT_OK; }
 
 } // extern "C"
