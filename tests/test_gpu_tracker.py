@@ -199,11 +199,12 @@ def test_full_size_properties_512(built, frames):
     assert results[0] == results[1]                                                              # cyclic offset changes storage, not content
 
 
-@pytest.mark.parametrize("odometry", [0, 2])
+@pytest.mark.parametrize("odometry", [0, 1, 2])
 def test_prefetch_hint_does_not_change_results(built, frames, odometry):
-    """kt_prefetch_frame moves the copy AND the pose-independent front end of the next frame (scaleDepth, bilateral, pyramid, maps) onto a
-    side stream, into a spare buffer set.  Results must be bit-identical with the hint, without it, and with hints given only for some
-    frames -- including the stale y/z planes of invalid map pixels (Q7) that the colour integration can read, hence the depth holes."""
+    """kt_prefetch_frame moves the copy AND the pose-independent front end of the next frame (scaleDepth, bilateral, pyramid, maps, and
+    for -r / -ri the photometric pyramids) onto a side stream, into a spare buffer set.  Results must be bit-identical with the hint,
+    without it, with hints given only for some frames, and with a hint before the first frame (it copies the inputs only) -- including
+    the stale y/z planes of invalid map pixels (Q7) that the colour integration can read, hence the depth holes."""
     import torch
     import kintinuous_b200 as kb
     rng = np.random.default_rng(7)
@@ -218,9 +219,10 @@ def test_prefetch_hint_does_not_change_results(built, frames, odometry):
     dd = [t.cuda() for t in pd]; dc = [t.cuda() for t in pc]
     cfg = dict(vol=256, odometry=odometry, voxel_shift=4)
     ref = kb.Tracker(kb.Config.default(**cfg))
-    hinted = kb.Tracker(kb.Config.default(**cfg))             # hint before every frame, host pointers
+    hinted = kb.Tracker(kb.Config.default(**cfg))             # hint before every frame, the first included, host pointers
     mixed = kb.Tracker(kb.Config.default(**cfg))              # hint before some frames only, device pointers
     skip = {3, 6}
+    hinted.prefetch_frame(pd[0].data_ptr(), pc[0].data_ptr())
     for k in range(n):
         pa = ref.process_frame(fr[k][0], fr[k][1], k)
         pb = hinted.process_frame(pd[k].data_ptr(), pc[k].data_ptr(), k)
@@ -231,12 +233,18 @@ def test_prefetch_hint_does_not_change_results(built, frames, odometry):
                 mixed.prefetch_frame(dd[k + 1], dc[k + 1])
         for p in (pb, pm):
             assert list(pa.t) == list(p.t) and list(pa.R) == list(p.R) and list(pa.voxel_wrap) == list(p.voxel_wrap), k
+    # every buffer kt_download_map exposes that the mode writes.  -r ray-casts one level, and builds no depth pyramid, maps or colour
+    # inputs (Q10): those buffers are never written, and the depth pyramid and colour inputs never zeroed either.
+    if odometry == 1:
+        taps = [(which, 0) for which in (2, 3, 5, 6)]
+    else:
+        taps = [(which, level) for which in range(5) for level in range(4)] + [(which, 0) for which in (5, 6, 7, 8)]
     ta, ca = ref.export_volume()
     for trk in (hinted, mixed):
         tb, cb = trk.export_volume()
         assert (ta == tb).all() and (ca == cb).all()
-        for which in (0, 1, 2, 3):
-            assert np.array_equal(ref.download_map(which, 0), trk.download_map(which, 0), equal_nan=True)
+        for which, level in taps:
+            assert np.array_equal(ref.download_map(which, level), trk.download_map(which, level), equal_nan=True), (which, level)
         trk.close()
     ref.close()
 
