@@ -27,48 +27,66 @@ struct RayParams {
     float* peer_vmap[MAX_GPUS][LEVELS]; float* peer_nmap[MAX_GPUS][LEVELS]; uchar4* peer_vcol[MAX_GPUS];
 };
 
+// 1 / x as the build's division (div.full.f32 under --prec-div=false, FTZ) computes it for |x| <= 2^126: MUFU.RCP.  The division
+// itself is x * rcp(y) for such y, so a quotient by the cell size is __fmul_rn(x, rcp_approx(cell)) bit for bit; raycast() refuses a
+// cell size outside that range, and tests/test_gpu_raycast_rcp.py checks the identity on the device.
+__device__ __forceinline__ float rcp_approx(float x)
+{
+    float r;
+    asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(r) : "f"(x));
+    return r;
+}
+
+// One axis of a trilinear tap at coordinate x: v = the voxel holding x, g = the lower voxel of the two the tap blends (v, or v - 1
+// when x lies below v's centre) and f = the weight of g + 1.
+struct Axis { int v; int g; float f; };
+
 // POW2: V is a power of two (cyclic wrap by mask, plane / row offsets by shift); IdxT: 32-bit voxel index when V^3 <= 2^31.
 template <bool POW2, typename IdxT, bool MG = false>
 struct Caster {
     const RayParams& p;
     int shift;
-    __device__ __forceinline__ Caster(const RayParams& p_) : p(p_) { shift = POW2 ? (31 - __clz(p_.V)) : 0; }
-
-    __device__ __forceinline__ IdxT addr(int x, int y, int z) const
+    float3 inv;             // 1 / cell_size, once per ray
+    __device__ __forceinline__ Caster(const RayParams& p_) : p(p_)
     {
-        if (POW2) {
-            const int m = p.V - 1;
-            const unsigned int sx = (x + p.wrap.x) & m, sy = (y + p.wrap.y) & m, sz = (z + p.wrap.z) & m;
-            return ((((IdxT)sz << shift) | sy) << shift) | sx;
-        }
-        int sx = x + p.wrap.x; if (sx >= p.V) sx -= p.V;
-        int sy = y + p.wrap.y; if (sy >= p.V) sy -= p.V;
-        int sz = z + p.wrap.z; if (sz >= p.V) sz -= p.V;
+        shift = POW2 ? (31 - __clz(p_.V)) : 0;
+        inv = make_float3(rcp_approx(p_.cell_size.x), rcp_approx(p_.cell_size.y), rcp_approx(p_.cell_size.z));
+    }
+
+    __device__ __forceinline__ unsigned int wrap1(int x, int w) const
+    {
+        if (POW2) return (unsigned int)(x + w) & (unsigned int)(p.V - 1);
+        int s = x + w; if (s >= p.V) s -= p.V;
+        return (unsigned int)s;
+    }
+    // the storage coordinate after wrap1(x, w): wrap1(x + 1, w) for x + 1 < V
+    __device__ __forceinline__ unsigned int next1(unsigned int s) const
+    {
+        if (POW2) return (s + 1) & (unsigned int)(p.V - 1);
+        return (s + 1 == (unsigned int)p.V) ? 0u : s + 1;
+    }
+    __device__ __forceinline__ IdxT index(unsigned int sx, unsigned int sy, unsigned int sz) const
+    {
+        if (POW2) return ((((IdxT)sz << shift) | sy) << shift) | sx;
         return ((IdxT)sz * p.V + sy) * p.V + sx;
     }
     // shared volume (MG): the TSDF is replicated, so the march and every trilinear TSDF tap read LOCAL memory exactly as on one GPU; only
     // the colour / weight planes are sharded (block-cyclic by storage z): local memory or an NVLink peer (CUDA IPC) through the table
     __device__ __forceinline__ short rawTsdf(int x, int y, int z) const
     {
-        return __ldg(&p.volume[addr(x, y, z)]);
+        return __ldg(&p.volume[index(wrap1(x, p.wrap.x), wrap1(y, p.wrap.y), wrap1(z, p.wrap.z))]);
     }
-    __device__ __forceinline__ float readTsdf(int x, int y, int z) const { return unpack_tsdf(rawTsdf(x, y, z)); }
-    __device__ __forceinline__ uchar4 readColor(int x, int y, int z) const
+    __device__ __forceinline__ const uchar4* colorPlane(unsigned int sz) const
     {
-        if (MG) {
-            const int m = p.V - 1;
-            const unsigned int sx = (x + p.wrap.x) & m, sy = (y + p.wrap.y) & m, sz = (z + p.wrap.z) & m;
-            const unsigned int lz = (unsigned int)vv_local_plane(p.vv, (int)sz);
-            return __ldg(reinterpret_cast<const uchar4*>(p.vv.color[vv_owner(p.vv, (int)sz)]) + ((((size_t)lz << shift) | sy) << shift | sx));
-        }
-        return __ldg(&p.color_volume[addr(x, y, z)]);
+        if (MG) return reinterpret_cast<const uchar4*>(p.vv.color[vv_owner(p.vv, (int)sz)]) + ((size_t)vv_local_plane(p.vv, (int)sz) << (2 * shift));
+        return p.color_volume + (size_t)index(0, 0, sz);
     }
 
     __device__ __forceinline__ int3 getVoxel(float3 point) const
     {
-        int vx = __float2int_rd(point.x / p.cell_size.x);
-        int vy = __float2int_rd(point.y / p.cell_size.y);
-        int vz = __float2int_rd(point.z / p.cell_size.z);
+        int vx = __float2int_rd(__fmul_rn(point.x, inv.x));
+        int vy = __float2int_rd(__fmul_rn(point.y, inv.y));
+        int vz = __float2int_rd(__fmul_rn(point.z, inv.z));
         return make_int3(vx, vy, vz);
     }
     __device__ __forceinline__ bool checkInds(const int3& g) const
@@ -76,57 +94,75 @@ struct Caster {
         return ((unsigned)g.x < (unsigned)p.V && (unsigned)g.y < (unsigned)p.V && (unsigned)g.z < (unsigned)p.V);
     }
 
-    // trilinear weights and base voxel of a point; false if the base voxel is outside [1, V-2]
-    __device__ __forceinline__ bool trilinearSetup(const float3& point, int3& g, float& a, float& b, float& c) const
+    __device__ __forceinline__ Axis axis(float x, float cell, float r) const
     {
-        g = getVoxel(point);
-        if (g.x <= 0 || g.x >= p.V - 1) return false;
-        if (g.y <= 0 || g.y >= p.V - 1) return false;
-        if (g.z <= 0 || g.z >= p.V - 1) return false;
-        float vx = (g.x + 0.5f) * p.cell_size.x;
-        float vy = (g.y + 0.5f) * p.cell_size.y;
-        float vz = (g.z + 0.5f) * p.cell_size.z;
-        g.x = (point.x < vx) ? (g.x - 1) : g.x;
-        g.y = (point.y < vy) ? (g.y - 1) : g.y;
-        g.z = (point.z < vz) ? (g.z - 1) : g.z;
-        a = __fmaf_rn(-(g.x + 0.5f), p.cell_size.x, point.x) / p.cell_size.x;        // (point.x - (g.x + 0.5f) * cell.x) / cell.x
-        b = __fmaf_rn(-(g.y + 0.5f), p.cell_size.y, point.y) / p.cell_size.y;
-        c = __fmaf_rn(-(g.z + 0.5f), p.cell_size.z, point.z) / p.cell_size.z;
-        return true;
+        Axis s;
+        s.v = __float2int_rd(__fmul_rn(x, r));
+        s.g = (x < __fmul_rn(s.v + 0.5f, cell)) ? (s.v - 1) : s.v;
+        s.f = __fmul_rn(__fmaf_rn(-(s.g + 0.5f), cell, x), r);      // (x - (g + 0.5f) * cell) / cell
+        return s;
+    }
+    __device__ __forceinline__ Axis axisX(float x) const { return axis(x, p.cell_size.x, inv.x); }
+    __device__ __forceinline__ Axis axisY(float y) const { return axis(y, p.cell_size.y, inv.y); }
+    __device__ __forceinline__ Axis axisZ(float z) const { return axis(z, p.cell_size.z, inv.z); }
+    // a tap is defined when the voxel of the point is inside [1, V-2] on every axis
+    __device__ __forceinline__ bool inner(const Axis& x, const Axis& y, const Axis& z) const
+    {
+        return x.v > 0 && x.v < p.V - 1 && y.v > 0 && y.v < p.V - 1 && z.v > 0 && z.v < p.V - 1;
     }
 
-    __device__ __forceinline__ float interpolateTrilineary(const float3& point) const
+    // readTsdf(000)*(1-a)*(1-b)*(1-c) + readTsdf(001)*(1-a)*(1-b)*c + ... + readTsdf(111)*a*b*c  (ray_caster.cu:155-171), written in the
+    // contraction nvcc gives that expression: every term's last multiply is fused into the running sum, except the second term,
+    // which is a plain product (fma(x0, w0, x1 * w1), then fma(xk, wk, sum)).  The eight addresses come from two wrapped
+    // coordinates per axis.
+    __device__ __forceinline__ float interpolateTrilineary(const Axis& x, const Axis& y, const Axis& z) const
     {
-        int3 g; float a, b, c;
-        if (!trilinearSetup(point, g, a, b, c)) return qnan();
-        float res = readTsdf(g.x + 0, g.y + 0, g.z + 0) * (1 - a) * (1 - b) * (1 - c) +
-                    readTsdf(g.x + 0, g.y + 0, g.z + 1) * (1 - a) * (1 - b) * c +
-                    readTsdf(g.x + 0, g.y + 1, g.z + 0) * (1 - a) * b * (1 - c) +
-                    readTsdf(g.x + 0, g.y + 1, g.z + 1) * (1 - a) * b * c +
-                    readTsdf(g.x + 1, g.y + 0, g.z + 0) * a * (1 - b) * (1 - c) +
-                    readTsdf(g.x + 1, g.y + 0, g.z + 1) * a * (1 - b) * c +
-                    readTsdf(g.x + 1, g.y + 1, g.z + 0) * a * b * (1 - c) +
-                    readTsdf(g.x + 1, g.y + 1, g.z + 1) * a * b * c;
+        if (!inner(x, y, z)) return qnan();
+        const unsigned int x0 = wrap1(x.g, p.wrap.x), x1 = next1(x0);
+        const unsigned int y0 = wrap1(y.g, p.wrap.y), y1 = next1(y0);
+        const unsigned int z0 = wrap1(z.g, p.wrap.z), z1 = next1(z0);
+        const int16_t* v = p.volume;
+        const float a = x.f, b = y.f, c = z.f;
+        const float a1 = 1 - a, b1 = 1 - b, c1 = 1 - c;
+        float res = __fmaf_rn(__fmul_rn(__fmul_rn(unpack_tsdf(__ldg(&v[index(x0, y0, z0)])), a1), b1), c1,
+                              __fmul_rn(__fmul_rn(__fmul_rn(unpack_tsdf(__ldg(&v[index(x0, y0, z1)])), a1), b1), c));
+        res = __fmaf_rn(__fmul_rn(__fmul_rn(unpack_tsdf(__ldg(&v[index(x0, y1, z0)])), a1), b), c1, res);
+        res = __fmaf_rn(__fmul_rn(__fmul_rn(unpack_tsdf(__ldg(&v[index(x0, y1, z1)])), a1), b), c, res);
+        res = __fmaf_rn(__fmul_rn(__fmul_rn(unpack_tsdf(__ldg(&v[index(x1, y0, z0)])), a), b1), c1, res);
+        res = __fmaf_rn(__fmul_rn(__fmul_rn(unpack_tsdf(__ldg(&v[index(x1, y0, z1)])), a), b1), c, res);
+        res = __fmaf_rn(__fmul_rn(__fmul_rn(unpack_tsdf(__ldg(&v[index(x1, y1, z0)])), a), b), c1, res);
+        res = __fmaf_rn(__fmul_rn(__fmul_rn(unpack_tsdf(__ldg(&v[index(x1, y1, z1)])), a), b), c, res);
         return res;
     }
 
     // colour (r,g,b truncated to u8) and weight ("heat") trilinear taps share the 8 uchar4 loads
-    __device__ __forceinline__ uchar4 interpolateColorHeat(const float3& point) const
+    __device__ __forceinline__ uchar4 interpolateColorHeat(const Axis& x, const Axis& y, const Axis& z) const
     {
-        int3 g; float a, b, c;
-        if (!trilinearSetup(point, g, a, b, c)) {
+        if (!inner(x, y, z)) {
             // interpolateColorTrilineary returns black, interpolateHeatTrilineary NaN -> (unsigned char)NaN
             uchar4 r; r.x = 0; r.y = 0; r.z = 0; r.w = (unsigned char)qnan();
             return r;
         }
-        const uchar4 c000 = readColor(g.x + 0, g.y + 0, g.z + 0), c001 = readColor(g.x + 0, g.y + 0, g.z + 1);
-        const uchar4 c010 = readColor(g.x + 0, g.y + 1, g.z + 0), c011 = readColor(g.x + 0, g.y + 1, g.z + 1);
-        const uchar4 c100 = readColor(g.x + 1, g.y + 0, g.z + 0), c101 = readColor(g.x + 1, g.y + 0, g.z + 1);
-        const uchar4 c110 = readColor(g.x + 1, g.y + 1, g.z + 0), c111 = readColor(g.x + 1, g.y + 1, g.z + 1);
-#define KT_TRI(f) ((float)c000.f * (1 - a) * (1 - b) * (1 - c) + (float)c001.f * (1 - a) * (1 - b) * c + \
-                   (float)c010.f * (1 - a) * b * (1 - c) + (float)c011.f * (1 - a) * b * c + \
-                   (float)c100.f * a * (1 - b) * (1 - c) + (float)c101.f * a * (1 - b) * c + \
-                   (float)c110.f * a * b * (1 - c) + (float)c111.f * a * b * c)
+        const unsigned int x0 = wrap1(x.g, p.wrap.x), x1 = next1(x0);
+        const unsigned int y0 = wrap1(y.g, p.wrap.y), y1 = next1(y0);
+        const unsigned int z0 = wrap1(z.g, p.wrap.z), z1 = next1(z0);
+        const uchar4* pz0 = colorPlane(z0);
+        const uchar4* pz1 = colorPlane(z1);
+        const uchar4 c000 = __ldg(pz0 + index(x0, y0, 0)), c001 = __ldg(pz1 + index(x0, y0, 0));
+        const uchar4 c010 = __ldg(pz0 + index(x0, y1, 0)), c011 = __ldg(pz1 + index(x0, y1, 0));
+        const uchar4 c100 = __ldg(pz0 + index(x1, y0, 0)), c101 = __ldg(pz1 + index(x1, y0, 0));
+        const uchar4 c110 = __ldg(pz0 + index(x1, y1, 0)), c111 = __ldg(pz1 + index(x1, y1, 0));
+        const float a = x.f, b = y.f, c = z.f;
+        // same 8-term trilinear sum as interpolateTrilineary, same contraction
+        const float a1 = 1 - a, b1 = 1 - b, c1 = 1 - c;
+#define KT_TRI(f) __fmaf_rn(__fmul_rn(__fmul_rn((float)c111.f, a), b), c, \
+                  __fmaf_rn(__fmul_rn(__fmul_rn((float)c110.f, a), b), c1, \
+                  __fmaf_rn(__fmul_rn(__fmul_rn((float)c101.f, a), b1), c, \
+                  __fmaf_rn(__fmul_rn(__fmul_rn((float)c100.f, a), b1), c1, \
+                  __fmaf_rn(__fmul_rn(__fmul_rn((float)c011.f, a1), b), c, \
+                  __fmaf_rn(__fmul_rn(__fmul_rn((float)c010.f, a1), b), c1, \
+                  __fmaf_rn(__fmul_rn(__fmul_rn((float)c000.f, a1), b1), c1, \
+                            __fmul_rn(__fmul_rn(__fmul_rn((float)c001.f, a1), b1), c))))))))
         uchar4 r;
         r.x = KT_TRI(x); r.y = KT_TRI(y); r.z = KT_TRI(z);
         float heat = KT_TRI(w);
@@ -197,8 +233,11 @@ __device__ __forceinline__ void cast_ray(const RayParams& p, int x, int y, bool&
     const float max_time = 3 * (p.volume_size.x + p.volume_size.y + p.volume_size.z);
     // The march (ray_caster.cu:345-425) is evaluated strictly in order, but the nearest-voxel reads of the next RS steps are
     // issued together: a step only needs the previous TSDF value to DECIDE, not to ADDRESS, so RS dependent L2 round trips
-    // become one.  time_curr advances by the same sequence of float additions as the reference's for-loop.
-    bool done = false;
+    // become one.  time_curr advances by the same sequence of float additions as the reference's for-loop.  The loop only
+    // finds the step tc of a +/- crossing; everything the surface needs is recomputed from tc below, so no voxel of the batch
+    // stays live across the decisions.
+    bool done = false, hit = false;
+    float tc = 0.f;
     while (!done && time_curr < max_time) {
         float tq[RS]; bool inb[RS]; short raw[RS];
         float t = time_curr;
@@ -213,43 +252,51 @@ __device__ __forceinline__ void cast_ray(const RayParams& p, int x, int y, bool&
 #pragma unroll
         for (int s = 0; s < RS; ++s) {
             if (done) break;
-            const float tc = tq[s];
-            if (!(tc < max_time)) { done = true; break; }
+            if (!(tq[s] < max_time)) { done = true; break; }
             const int tsdf_prev = tsdf;
             if (!inb[s]) { done = true; break; }
             tsdf = raw[s];
             if (tsdf_prev < 0 && tsdf > 0) { done = true; break; }
-            if (tsdf_prev > 0 && tsdf < 0) {
-                done = true;
-                float Ftdt = rc.interpolateTrilineary(ray_at(ray_start, ray_dir, (tc + time_step)));
-                if (isnan(Ftdt)) break;
-                float Ft = rc.interpolateTrilineary(ray_at(ray_start, ray_dir, tc));
-                if (isnan(Ft)) break;
-
-                float Ts = tc - time_step * Ft / (Ftdt - Ft);
-                float3 vetex_found = ray_at(ray_start, ray_dir, Ts);
-                vtx = vetex_found; v_ok = true;
-
-                int3 gc = rc.getVoxel(ray_at(ray_start, ray_dir, tc));
-                col = rc.interpolateColorHeat(vetex_found); c_ok = true;
-
-                if (gc.x > 1 && gc.y > 1 && gc.z > 1 && gc.x < p.V - 2 && gc.y < p.V - 2 && gc.z < p.V - 2) {
-                    float3 tt, n;
-                    tt = vetex_found; tt.x += p.cell_size.x; float Fx1 = rc.interpolateTrilineary(tt);
-                    tt = vetex_found; tt.x -= p.cell_size.x; float Fx2 = rc.interpolateTrilineary(tt);
-                    n.x = (Fx1 - Fx2);
-                    tt = vetex_found; tt.y += p.cell_size.y; float Fy1 = rc.interpolateTrilineary(tt);
-                    tt = vetex_found; tt.y -= p.cell_size.y; float Fy2 = rc.interpolateTrilineary(tt);
-                    n.y = (Fy1 - Fy2);
-                    tt = vetex_found; tt.z += p.cell_size.z; float Fz1 = rc.interpolateTrilineary(tt);
-                    tt = vetex_found; tt.z -= p.cell_size.z; float Fz2 = rc.interpolateTrilineary(tt);
-                    n.z = (Fz1 - Fz2);
-                    nrm = normalized3(n); n_ok = true;
-                }
-                break;
-            }
+            if (tsdf_prev > 0 && tsdf < 0) { done = true; hit = true; tc = tq[s]; break; }
         }
         time_curr = t;
+    }
+    if (!hit) return;
+
+    const float3 pn = ray_at(ray_start, ray_dir, (tc + time_step));
+    float Ftdt = rc.interpolateTrilineary(rc.axisX(pn.x), rc.axisY(pn.y), rc.axisZ(pn.z));
+    if (isnan(Ftdt)) return;
+    const float3 pc = ray_at(ray_start, ray_dir, tc);
+    const Axis cx = rc.axisX(pc.x), cy = rc.axisY(pc.y), cz = rc.axisZ(pc.z);
+    float Ft = rc.interpolateTrilineary(cx, cy, cz);
+    if (isnan(Ft)) return;
+
+    // tc - time_step * Ft / (Ftdt - Ft) as the build executes it: the division's rescale of a divisor above 2^126 by 1/4,
+    // then its multiply by the reciprocal fused into the subtraction
+    float num = __fmul_rn(time_step, Ft), den = __fsub_rn(Ftdt, Ft);
+    if (fabsf(den) > 0x1p126f) { num = __fmul_rn(num, 0.25f); den = __fmul_rn(den, 0.25f); }
+    float Ts = __fmaf_rn(-num, rcp_approx(den), tc);
+    const float3 vetex_found = ray_at(ray_start, ray_dir, Ts);
+    vtx = vetex_found; v_ok = true;
+
+    // the vertex's per-axis set-up serves the colour tap as it is, and each normal tap for the two axes it does not move
+    const Axis vx = rc.axisX(vetex_found.x), vy = rc.axisY(vetex_found.y), vz = rc.axisZ(vetex_found.z);
+    col = rc.interpolateColorHeat(vx, vy, vz); c_ok = true;
+
+    // the voxel of the ray at tc
+    if (cx.v > 1 && cy.v > 1 && cz.v > 1 && cx.v < p.V - 2 && cy.v < p.V - 2 && cz.v < p.V - 2) {
+        float3 n;
+        float F1 = rc.interpolateTrilineary(rc.axisX(__fadd_rn(vetex_found.x, p.cell_size.x)), vy, vz);
+        float F2 = rc.interpolateTrilineary(rc.axisX(__fsub_rn(vetex_found.x, p.cell_size.x)), vy, vz);
+        n.x = __fsub_rn(F1, F2);
+        F1 = rc.interpolateTrilineary(vx, rc.axisY(__fadd_rn(vetex_found.y, p.cell_size.y)), vz);
+        F2 = rc.interpolateTrilineary(vx, rc.axisY(__fsub_rn(vetex_found.y, p.cell_size.y)), vz);
+        n.y = __fsub_rn(F1, F2);
+        F1 = rc.interpolateTrilineary(vx, vy, rc.axisZ(__fadd_rn(vetex_found.z, p.cell_size.z)));
+        F2 = rc.interpolateTrilineary(vx, vy, rc.axisZ(__fsub_rn(vetex_found.z, p.cell_size.z)));
+        n.z = __fsub_rn(F1, F2);
+        const float rn = rsqrtf(dot3(n, n));                                       // normalized3(n)
+        nrm = make_float3(__fmul_rn(n.x, rn), __fmul_rn(n.y, rn), __fmul_rn(n.z, rn)); n_ok = true;
     }
 }
 
@@ -385,6 +432,9 @@ int raycast(const RaycastArgs& a, cudaStream_t s)
     for (int l = 0; l < LEVELS; ++l) { p.vmap[l] = a.vmap[l]; p.nmap[l] = a.nmap[l]; }
     p.vmap_color = (uchar4*)a.vmap_color; p.rows = a.rows; p.cols = a.cols;
     p.n_levels = a.n_levels; p.z_begin = 0; p.tile_row_begin = 0; p.n_out = 1;
+    // every quotient by the cell size is a multiply by its reciprocal (rcp_approx), which equals the division only up to 2^126
+    const float3 cs = p.cell_size;
+    if (!(fabsf(cs.x) <= 0x1p126f && fabsf(cs.y) <= 0x1p126f && fabsf(cs.z) <= 0x1p126f)) { set_error("raycast: cell size (volume_size / vol) must be finite and at most 2^126"); return -1; }
     // the in-tile pyramid needs every level's tile to be whole
     if (p.n_levels > 1 && ((a.cols % RC_X) != 0 || (a.rows % RC_Y) != 0)) { set_error("raycast: fused pyramid needs cols %% 16 == 0 and rows %% 8 == 0"); return -1; }
     dim3 block(RC_X, RC_Y), grid(div_up(a.cols, RC_X), div_up(a.rows, RC_Y));
