@@ -152,6 +152,12 @@ KT_API int kt_get_slice_mesh(kt_ctx* ctx, int idx, kt_mesh_vertex* verts, size_t
 /* The whole volume's mesh at this moment, synchronous, without recording a slice (the live mesh of PangoVis.cpp:395), with the weight
  * cull of kt_set_slice_meshing (8 until it is called); copies up to the capacities, returns both counts.  world > 1: KT_ERR_INVALID. */
 KT_API int kt_get_live_mesh(kt_ctx* ctx, kt_mesh_vertex* verts, size_t max_verts, uint32_t* tris, size_t max_tris, size_t* n_verts, size_t* n_tris);
+/* Where slice idx's mesh sits on the global voxel lattice (the keys kt_get_map_mesh welds by): per vertex (gx, gy, gz, axis), the lower
+ * voxel and axis of the edge it lies on; per triangle (gx, gy, gz, 0), the lower corner of its cell -- the logical voxel plus the slice's
+ * real voxel wrap, the world voxel index the positions are computed from (kt_op_mesh_volume_keyed).  Copies up to max_verts / max_tris
+ * records of 4 int32 (the counts are kt_get_slice_mesh's); waits for that slice's download only.  KT_ERR_STATE for a slice recorded
+ * with meshing off. */
+KT_API int kt_get_slice_mesh_keys(kt_ctx* ctx, int idx, int32_t* vert_edges, size_t max_verts, int32_t* tri_cells, size_t max_tris);
 /* MeshGenerator::save's "merging for export" branch (:229-280): every recorded slice mesh in order, indices offset, as one binary
  * little-endian PLY (vertex: float x y z nx ny nz, uchar red green blue; face: list uchar int vertex_indices).  KT_ERR_STATE when no
  * recorded slice has a mesh. */
@@ -229,6 +235,34 @@ typedef struct kt_map_report {
 } kt_map_report;
 KT_API int kt_get_map_cloud(kt_ctx* ctx, int which, int dedupe, kt_point_xyzrgbnormal* out, size_t capacity, size_t* count, kt_map_report* report);
 KT_API int kt_save_map_pcd(kt_ctx* ctx, const char* path, int which, int dedupe, kt_map_report* report);
+/* The map as one mesh, the mesh half of the export above (the reference's MeshGenerator::save, MeshGenerator.cpp:37-191).
+ *   which = 0: every slice mesh recorded with meshing on since the last reset, in order, the FINAL slice of kt_finalise included.
+ *   which = 1: the corrected map, as kt_get_map_cloud's: slices covered by the last kt_deform_map / kt_close_loop contribute their
+ *     deformed vertices (kt_get_deformed_slice_mesh); later slices are moved rigidly by the same C (positions R x + t, normals R n, FP32
+ *     on the device).  The triangles are which 0's.  KT_ERR_STATE before any deformation or after kt_reset.
+ *   weld = 0: the concatenation with offset indices (kt_save_mesh_ply's content).
+ *   weld = 1: kt_op_weld_meshes over the slice meshes and their keys (kt_get_slice_mesh_keys): every global cell keeps the triangles
+ *     of the latest slice that meshed it (its TSDF has fused the most frames), every global edge one vertex, so the overlap planes
+ *     neighbouring slices share appear once and the seams are connected.  Where two slices disagree about the sign of a shared corner
+ *     (the surface moved between them) a gap one cell wide is left; there is no hole filling.
+ * Copies up to max_verts / max_tris (NULL outputs: counts only) and returns both counts; every call redoes the work.  Waits for slice
+ * downloads still in flight and works on the slice stream between frames: tracking reads nothing it writes.  KT_ERR_STATE when no slice
+ * was recorded with meshing on; KT_ERR_INVALID for a volume shared by several GPUs; KT_ERR_CUDA when device memory for the export cannot
+ * be allocated.  kt_save_map_ply writes the same mesh in kt_save_mesh_ply's binary PLY layout; the reference's "-nos" mesh is
+ * (which 0, weld 1). */
+typedef struct kt_weld_report {
+    size_t input_verts, input_tris;     /* of the concatenation */
+    size_t output_verts, output_tris;   /* of the exported mesh */
+    size_t repeated_cells;              /* weld: cells that more than one mesh has triangles in */
+    size_t dropped_triangles;           /* weld: triangles in a cell another, later mesh also meshed */
+    size_t merged_vertices;             /* weld: vertices kept triangles use that share their edge with a later mesh's vertex */
+    int meshes;                         /* slices (meshes) in the concatenation */
+    int moved_meshes;                   /* slices placed by the rigid correction (which = 1) */
+    float upload_ms, sort_ms, weld_ms, download_ms, total_ms;      /* CUDA-event times of the device work (0 without any) */
+} kt_weld_report;
+KT_API int kt_get_map_mesh(kt_ctx* ctx, int which, int weld, kt_mesh_vertex* verts, size_t max_verts, uint32_t* tris, size_t max_tris,
+                           size_t* n_verts, size_t* n_tris, kt_weld_report* report);
+KT_API int kt_save_map_ply(kt_ctx* ctx, const char* path, int which, int weld, kt_weld_report* report);
 /* Loop closure: the pose-graph half of the reference's backend (backend/Deformation.cpp:130-346 addCameraCamera / addCameraLoop,
  * backend/iSAMInterface.cpp) on the GPU.  The caller passes what PlaceRecognition produces (LoopClosureConstraint,
  * PlaceRecognition.cpp:198-209): time1 (the new frame) and time2 (the old one), both dense pose timestamps, the pose of the camera at
@@ -457,6 +491,33 @@ KT_API int kt_op_mesh_volume(const int16_t* tsdf_dev, const uint8_t* color_dev, 
                              const int* voxel_wrap3, const int* real_voxel_wrap3, int minX, int maxX, int minY, int maxY, int minZ, int maxZ,
                              int weight_cull, kt_mesh_vertex* verts_dev, size_t max_verts, uint32_t* tris_dev, size_t max_tris,
                              size_t* n_verts, size_t* n_tris, void* stream);
+/* kt_op_mesh_volume that also says where each vertex and triangle is on the global voxel lattice: vert_edges_dev gets (gx, gy, gz, axis)
+ * per vertex, the lower voxel and axis of its edge, and tri_cells_dev (gx, gy, gz, 0) per triangle, the lower corner of its cell, both
+ * int32 x 4 and global = logical voxel + real_voxel_wrap3.  Vertices and triangles are byte-identical to kt_op_mesh_volume's, with the
+ * same capacity contract (max_verts bounds vert_edges_dev too, max_tris tri_cells_dev). */
+KT_API int kt_op_mesh_volume_keyed(const int16_t* tsdf_dev, const uint8_t* color_dev, int vol, const float* volume_size3,
+                                   const int* voxel_wrap3, const int* real_voxel_wrap3, int minX, int maxX, int minY, int maxY, int minZ, int maxZ,
+                                   int weight_cull, kt_mesh_vertex* verts_dev, int32_t* vert_edges_dev, size_t max_verts, uint32_t* tris_dev,
+                                   int32_t* tri_cells_dev, size_t max_tris, size_t* n_verts, size_t* n_tris, void* stream);
+/* Weld n_meshes keyed meshes (kt_op_mesh_volume_keyed, kt_get_slice_mesh_keys) into one (kt_weld.cu).  Input (device): the meshes
+ * concatenated in order -- vertices with their edges, triangles (indices local to their own mesh) with their cells -- and n_meshes + 1
+ * HOST offsets of each mesh's first vertex / triangle (vert_offsets_host[n_meshes] = all vertices).
+ *   - Cell winner: every global cell keeps the triangles of the highest-numbered mesh that has triangles there; a cell only one mesh
+ *     meshed keeps that mesh's.
+ *   - Vertex weld: only vertices a kept triangle uses are kept; of those on one global edge, the highest-numbered mesh's (32 bytes
+ *     copied unchanged) represents them all.
+ *   - Order: vertices ascend by (gz, gy, gx, axis), triangles by cell (gz, gy, gx) and within a cell in the winning mesh's order; indices
+ *     point into the output.  This is kt_op_mesh_volume's order, so welding keyed meshes of overlapping boxes of one volume gives exactly
+ *     the union box's mesh.  Deterministic: two calls give byte-identical output.
+ * No triangles in: nothing out.  KT_ERR_INVALID for n_meshes < 1, null or descending offsets, more than 2^31 - 1 vertices or triangles
+ * in, an axis outside 0..2, an index outside its mesh, or keys beyond 2^62 (3 x the voxels of the lattice box the keys span);
+ * KT_ERR_CAPACITY when either output is too small (both counts returned, nothing written); KT_ERR_CUDA when its scratch cannot be
+ * allocated.  report (may be NULL): the counts, sort_ms /
+ * weld_ms / total_ms. */
+KT_API int kt_op_weld_meshes(const kt_mesh_vertex* verts_dev, const int32_t* vert_edges_dev, const size_t* vert_offsets_host,
+                             const uint32_t* tris_dev, const int32_t* tri_cells_dev, const size_t* tri_offsets_host, int n_meshes,
+                             kt_mesh_vertex* out_verts_dev, size_t max_verts, uint32_t* out_tris_dev, size_t max_tris, size_t* n_verts, size_t* n_tris,
+                             kt_weld_report* report, void* stream);
 /* Deformation graph operators (kt_deform_map runs the three in turn).  Nodes: n_nodes float xyz positions and their uint64 times,
  * ascending (device).  kind: 0 = kt_point_xyzrgbnormal, 1 = kt_mesh_vertex, 2 = packed float xyz (weights only).
  * kt_op_deform_weights -- weightVerticesSeq (DeformationGraph.cpp:441-556): per point, the node nearest its time by binary search (a time

@@ -156,6 +156,17 @@ class MapReport(C.Structure):
         return {k: getattr(self, k) for k, _ in self._fields_}
 
 
+class WeldReport(C.Structure):
+    """kt_weld_report of kt_get_map_mesh / kt_save_map_ply / kt_op_weld_meshes."""
+    _fields_ = [("input_verts", C.c_size_t), ("input_tris", C.c_size_t), ("output_verts", C.c_size_t), ("output_tris", C.c_size_t),
+                ("repeated_cells", C.c_size_t), ("dropped_triangles", C.c_size_t), ("merged_vertices", C.c_size_t), ("meshes", C.c_int),
+                ("moved_meshes", C.c_int), ("upload_ms", C.c_float), ("sort_ms", C.c_float), ("weld_ms", C.c_float),
+                ("download_ms", C.c_float), ("total_ms", C.c_float)]
+
+    def as_dict(self):
+        return {k: getattr(self, k) for k, _ in self._fields_}
+
+
 class SliceInfo(C.Structure):
     _fields_ = [("dimension", C.c_int), ("odometry", C.c_int), ("camera_t", C.c_float * 3), ("camera_R", C.c_float * 9),
                 ("utime", C.c_uint64), ("count", C.c_size_t)]
@@ -299,6 +310,34 @@ class Tracker:
         v = np.zeros(nv.value, MESH_VERTEX_DTYPE); t = np.zeros((nt.value, 3), np.uint32)
         _check(self.lib.kt_get_slice_mesh(self.h, idx, _ptr(v), C.c_size_t(len(v)), _ptr(t), C.c_size_t(len(t)), C.byref(nv), C.byref(nt)))
         return v, t
+
+    def get_slice_mesh_keys(self, idx):
+        """(vertex edges int32 [n, 4] = gx, gy, gz, axis; triangle cells int32 [m, 4] = gx, gy, gz, 0) of slice idx's mesh on the global
+        voxel lattice (kt_get_slice_mesh_keys)."""
+        nv = C.c_size_t(0); nt = C.c_size_t(0)
+        _check(self.lib.kt_get_slice_mesh(self.h, idx, None, C.c_size_t(0), None, C.c_size_t(0), C.byref(nv), C.byref(nt)))
+        e = np.zeros((nv.value, 4), np.int32); k = np.zeros((nt.value, 4), np.int32)
+        _check(self.lib.kt_get_slice_mesh_keys(self.h, idx, _ptr(e), C.c_size_t(len(e)), _ptr(k), C.c_size_t(len(k))))
+        return e, k
+
+    def map_mesh(self, which=0, weld=True):
+        """The map as one mesh (kt_get_map_mesh): which 0 = the recorded map, 1 = the corrected map; weld = every global cell and edge
+        once (the latest slice wins), else the slice meshes concatenated.  Returns (MESH_VERTEX_DTYPE [n], uint32 [m, 3], report dict).
+        Counts first, then fetches: that runs the export twice."""
+        nv = C.c_size_t(0); nt = C.c_size_t(0); rep = WeldReport()
+        _check(self.lib.kt_get_map_mesh(self.h, int(which), int(weld), None, C.c_size_t(0), None, C.c_size_t(0), C.byref(nv), C.byref(nt), C.byref(rep)))
+        v = np.zeros(nv.value, MESH_VERTEX_DTYPE); t = np.zeros((nt.value, 3), np.uint32)
+        if nv.value or nt.value:
+            _check(self.lib.kt_get_map_mesh(self.h, int(which), int(weld), _ptr(v), C.c_size_t(len(v)), _ptr(t), C.c_size_t(len(t)),
+                                            C.byref(nv), C.byref(nt), C.byref(rep)))
+        assert (nv.value, nt.value) == (len(v), len(t))
+        return v, t, rep.as_dict()
+
+    def save_map_ply(self, path, which=0, weld=True):
+        """The same mesh as a binary PLY in save_mesh_ply's layout (kt_save_map_ply).  Returns the report dict."""
+        rep = WeldReport()
+        _check(self.lib.kt_save_map_ply(self.h, os.fsencode(path), int(which), int(weld), C.byref(rep)))
+        return rep.as_dict()
 
     def live_mesh(self):
         """Mesh of the whole volume now (kt_get_live_mesh): (vertices, triangles)."""
@@ -645,6 +684,60 @@ class _Ops:
         _check(st)
         assert (nv2, nt2) == (nv, nt)
         return v.cpu().numpy().view(MESH_VERTEX_DTYPE).copy(), t[:3 * nt].cpu().numpy().view(np.uint32).reshape(nt, 3).copy()
+
+    def mesh_volume_keyed_into(self, tsdf, color, vol, volume_size, wrap, real_wrap, box, weight_cull, verts_dev, edges_dev, max_verts,
+                               tris_dev, cells_dev, max_tris):
+        """kt_op_mesh_volume_keyed into caller buffers: (status, n_verts, n_tris); status is 0 or KT_ERR_CAPACITY (nothing written)."""
+        vs = _f(volume_size)
+        w = np.ascontiguousarray(np.asarray(wrap, dtype=np.int32)); rw = np.ascontiguousarray(np.asarray(real_wrap, dtype=np.int32))
+        nv = C.c_size_t(0); nt = C.c_size_t(0)
+        st = self._l().kt_op_mesh_volume_keyed(_ptr(tsdf), _ptr(color), vol, _ptr(vs), _ptr(w), _ptr(rw), box[0], box[1], box[2], box[3], box[4],
+                                               box[5], int(weight_cull), _ptr(verts_dev), _ptr(edges_dev), C.c_size_t(max_verts), _ptr(tris_dev),
+                                               _ptr(cells_dev), C.c_size_t(max_tris), C.byref(nv), C.byref(nt), None)
+        if st not in (0, KT_ERR_CAPACITY):
+            _check(st)
+        return st, nv.value, nt.value
+
+    def mesh_volume_keyed(self, tsdf, color, vol, volume_size, wrap, real_wrap, box, weight_cull=8):
+        """mesh_volume plus where each vertex and triangle is: host arrays (vertices, triangles uint32 [m, 3], edges int32 [n, 4] = gx,
+        gy, gz, axis, cells int32 [m, 4] = gx, gy, gz, 0), global = logical voxel + real_wrap."""
+        import torch
+        st, nv, nt = self.mesh_volume_keyed_into(tsdf, color, vol, volume_size, wrap, real_wrap, box, weight_cull, None, None, 0, None, None, 0)
+        if st == 0:
+            return np.zeros(0, MESH_VERTEX_DTYPE), np.zeros((0, 3), np.uint32), np.zeros((0, 4), np.int32), np.zeros((0, 4), np.int32)
+        v = torch.empty(nv * 32, dtype=torch.uint8, device="cuda"); e = torch.empty(nv * 4, dtype=torch.int32, device="cuda")
+        t = torch.empty(max(nt, 1) * 3, dtype=torch.int32, device="cuda"); k = torch.empty(max(nt, 1) * 4, dtype=torch.int32, device="cuda")
+        st, nv2, nt2 = self.mesh_volume_keyed_into(tsdf, color, vol, volume_size, wrap, real_wrap, box, weight_cull, v, e, nv, t, k, nt)
+        _check(st)
+        assert (nv2, nt2) == (nv, nt)
+        return (v.cpu().numpy().view(MESH_VERTEX_DTYPE).copy(), t[:3 * nt].cpu().numpy().view(np.uint32).reshape(nt, 3).copy(),
+                e.cpu().numpy().reshape(nv, 4), k[:4 * nt].cpu().numpy().reshape(nt, 4))
+
+    def weld_meshes_into(self, verts_dev, edges_dev, vert_offsets, tris_dev, cells_dev, tri_offsets, out_verts_dev, max_verts, out_tris_dev, max_tris):
+        """kt_op_weld_meshes on device buffers with host offsets (n_meshes + 1 each): (status, n_verts, n_tris, report dict); status is 0
+        or KT_ERR_CAPACITY (nothing written)."""
+        vo = np.ascontiguousarray(np.asarray(vert_offsets, np.uint64)); to = np.ascontiguousarray(np.asarray(tri_offsets, np.uint64))
+        nv = C.c_size_t(0); nt = C.c_size_t(0); rep = WeldReport()
+        st = self._l().kt_op_weld_meshes(_ptr(verts_dev), _ptr(edges_dev), _ptr(vo), _ptr(tris_dev), _ptr(cells_dev), _ptr(to), len(vo) - 1,
+                                         _ptr(out_verts_dev), C.c_size_t(max_verts), _ptr(out_tris_dev), C.c_size_t(max_tris), C.byref(nv), C.byref(nt),
+                                         C.byref(rep), None)
+        if st not in (0, KT_ERR_CAPACITY):
+            _check(st)
+        return st, nv.value, nt.value, rep.as_dict()
+
+    def weld_meshes(self, meshes):
+        """Weld host meshes [(vertices, triangles [m, 3], edges [n, 4], cells [m, 4])] on the device: (vertices, triangles, report dict)."""
+        import torch
+        cat = lambda xs, dt, w: np.ascontiguousarray(np.concatenate([np.asarray(x, dt).reshape(-1, w) for x in xs]) if xs else np.zeros((0, w), dt))  # noqa: E731
+        v = np.concatenate([np.asarray(m[0]) for m in meshes]) if meshes else np.zeros(0, MESH_VERTEX_DTYPE)
+        t = cat([m[1] for m in meshes], np.uint32, 3); e = cat([m[2] for m in meshes], np.int32, 4); k = cat([m[3] for m in meshes], np.int32, 4)
+        vo = np.concatenate([[0], np.cumsum([len(m[0]) for m in meshes])]); to = np.concatenate([[0], np.cumsum([len(m[1]) for m in meshes])])
+        dev = lambda a: torch.from_numpy(np.ascontiguousarray(a).view(np.uint8).reshape(-1).copy()).cuda() if a.size else None  # noqa: E731
+        dv, dt, de, dk = dev(v), dev(t), dev(e), dev(k)
+        ov = torch.empty(max(len(v), 1) * 32, dtype=torch.uint8, device="cuda"); ot = torch.empty(max(len(t), 1) * 12, dtype=torch.uint8, device="cuda")
+        st, nv, nt, rep = self.weld_meshes_into(dv, de, vo, dt, dk, to, ov, len(v), ot, len(t))
+        _check(st)
+        return ov[:nv * 32].cpu().numpy().view(MESH_VERTEX_DTYPE).copy(), ot[:nt * 12].cpu().numpy().view(np.uint32).reshape(nt, 3).copy(), rep
 
     def deform_weights(self, node_pos, node_times, points, kind, times, ids, weights):
         """kt_op_deform_weights: node_pos float32 [n, 3], node_times uint64 [n] (as int64 tensors), points (kind 0

@@ -24,7 +24,7 @@ cudaStream_t st(void* s) { return (cudaStream_t)s; }
 // (the device current at the call), and the calls that use it are serialised by a process-wide mutex, so operator calls from several
 // host threads / on several devices are safe, just not concurrent.
 struct OpScratch { Allocations mem; OdomState* state; float* partials; int* ipartials; unsigned int* counter; OdomState* host_state;
-                   DeviceBuffer<float> ztable; SliceWorkspace slice_ws; MeshWorkspace mesh_ws; SurfWorkspace surf_ws; PnpWorkspace pnp_ws;
+                   DeviceBuffer<float> ztable; SliceWorkspace slice_ws; MeshWorkspace mesh_ws; DeviceBuffer<unsigned long long> mesh_cells; SurfWorkspace surf_ws; PnpWorkspace pnp_ws;
                    SliceWorkspace fit_ws; DeviceBuffer<int> place_ints; };   // place_ints: kt_op_surf / kt_op_match_ratio counts in, counts out
 enum { KT_MAX_DEVICES = 64 };
 // Allocated once per device and never destroyed: no CUDA call may run in the static destructors at process exit.
@@ -207,6 +207,40 @@ int kt_op_mesh_volume(const int16_t* tsdf, const uint8_t* color, int vol, const 
     r = mesh_emit(a, &g_ops.mesh_ws, nv, verts, tris, st(s)); if (r) return r;
     KT_CUDA(cudaStreamSynchronize(st(s)));
     return KT_OK;
+}
+
+int kt_op_mesh_volume_keyed(const int16_t* tsdf, const uint8_t* color, int vol, const float* vs, const int* wrap, const int* real_wrap,
+                            int minX, int maxX, int minY, int maxY, int minZ, int maxZ, int weight_cull, kt_mesh_vertex* verts, int32_t* vert_edges,
+                            size_t max_verts, uint32_t* tris, int32_t* tri_cells, size_t max_tris, size_t* n_verts, size_t* n_tris, void* s)
+{
+    if (!tsdf || !color || !vs || !wrap || !real_wrap || !n_verts || !n_tris || vol <= 0) { set_error("kt_op_mesh_volume_keyed: bad argument"); return KT_ERR_INVALID; }
+    if (minX < 0 || minY < 0 || minZ < 0 || maxX > vol || maxY > vol || maxZ > vol) { set_error("kt_op_mesh_volume_keyed: box outside [0, vol]"); return KT_ERR_INVALID; }
+    KT_OPS_LOCK();
+    MeshArgs a;
+    a.tsdf = tsdf; a.color = color; a.vol = vol; a.volume_size = make_float3(vs[0], vs[1], vs[2]);
+    a.wrap = make_int3(wrap[0], wrap[1], wrap[2]); a.real_wrap = make_int3(real_wrap[0], real_wrap[1], real_wrap[2]);
+    a.minX = minX; a.maxX = maxX; a.minY = minY; a.maxY = maxY; a.minZ = minZ; a.maxZ = maxZ; a.weight_cull = weight_cull;
+    size_t nv = 0, nt = 0;
+    int r = mesh_count(a, &g_ops.mesh_ws, &nv, &nt, st(s)); if (r) return r;
+    *n_verts = nv; *n_tris = nt;
+    if (nv > max_verts || nt > max_tris || (nv && (!verts || !vert_edges)) || (nt && (!tris || !tri_cells))) {
+        set_error("kt_op_mesh_volume_keyed: %zu vertices / %zu triangles exceed the capacities", nv, nt); return KT_ERR_CAPACITY;
+    }
+    if ((r = g_ops.mesh_cells.grow(nt, nt, "operator mesh cells"))) return r;
+    r = mesh_emit(a, &g_ops.mesh_ws, nv, verts, tris, st(s), nullptr, g_ops.mesh_cells.get()); if (r) return r;
+    if ((r = mesh_global_keys(a, g_ops.mesh_ws.keys.get(), nv, true, vert_edges, st(s)))) return r;
+    if ((r = mesh_global_keys(a, g_ops.mesh_cells.get(), nt, false, tri_cells, st(s)))) return r;
+    KT_CUDA(cudaStreamSynchronize(st(s)));
+    return KT_OK;
+}
+
+int kt_op_weld_meshes(const kt_mesh_vertex* verts, const int32_t* vert_edges, const size_t* vert_offsets, const uint32_t* tris, const int32_t* tri_cells,
+                      const size_t* tri_offsets, int n_meshes, kt_mesh_vertex* out_verts, size_t max_verts, uint32_t* out_tris, size_t max_tris,
+                      size_t* n_verts, size_t* n_tris, kt_weld_report* report, void* s)
+{
+    if (!n_verts || !n_tris) { set_error("kt_op_weld_meshes: bad argument"); return KT_ERR_INVALID; }
+    return weld_meshes(verts, vert_edges, vert_offsets, tris, tri_cells, tri_offsets, n_meshes, out_verts, max_verts, out_tris, max_tris, n_verts, n_tris,
+                       report, st(s));
 }
 
 int kt_op_deform_weights(const float* node_pos, const uint64_t* node_times, int n_nodes, const void* pts, int kind, const uint64_t* times,

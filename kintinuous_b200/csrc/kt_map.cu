@@ -170,6 +170,24 @@ map_rigid_kernel(kt_point_xyzrgbnormal* __restrict__ p, size_t n, const RigidF C
     }
 }
 
+// the same for kt_mesh_vertex records (x y z nx | ny nz rgba pad)
+__global__ void __launch_bounds__(MAP_THREADS)
+map_rigid_mesh_kernel(kt_mesh_vertex* __restrict__ p, size_t n, const RigidF C)
+{
+    for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
+        float4 a = reinterpret_cast<float4*>(p + i)[0], b = reinterpret_cast<float4*>(p + i)[1];
+        const float* R = C.R;
+        const float x = a.x, y = a.y, z = a.z, nx = a.w, ny = b.x, nz = b.y;
+        a.x = __fadd_rn(__fadd_rn(__fadd_rn(__fmul_rn(R[0], x), __fmul_rn(R[1], y)), __fmul_rn(R[2], z)), C.t[0]);
+        a.y = __fadd_rn(__fadd_rn(__fadd_rn(__fmul_rn(R[3], x), __fmul_rn(R[4], y)), __fmul_rn(R[5], z)), C.t[1]);
+        a.z = __fadd_rn(__fadd_rn(__fadd_rn(__fmul_rn(R[6], x), __fmul_rn(R[7], y)), __fmul_rn(R[8], z)), C.t[2]);
+        a.w = __fadd_rn(__fadd_rn(__fmul_rn(R[0], nx), __fmul_rn(R[1], ny)), __fmul_rn(R[2], nz));
+        b.x = __fadd_rn(__fadd_rn(__fmul_rn(R[3], nx), __fmul_rn(R[4], ny)), __fmul_rn(R[5], nz));
+        b.y = __fadd_rn(__fadd_rn(__fmul_rn(R[6], nx), __fmul_rn(R[7], ny)), __fmul_rn(R[8], nz));
+        reinterpret_cast<float4*>(p + i)[0] = a; reinterpret_cast<float4*>(p + i)[1] = b;
+    }
+}
+
 int grid_for(size_t n) { const size_t b = (n + MAP_THREADS - 1) / MAP_THREADS, cap = (size_t)device_info().sm_count * 16; return (int)(b < 1 ? 1 : (b > cap ? cap : b)); }
 
 // Stage timing of one voxel_grid call (CUDA events on its stream)
@@ -289,6 +307,14 @@ int rigid_move(void* points_dev, size_t n, const RigidF& C, cudaStream_t s)
 {
     if (!n) return 0;
     map_rigid_kernel<<<grid_for(n), MAP_THREADS, 0, s>>>((kt_point_xyzrgbnormal*)points_dev, n, C);
+    KT_LAUNCH_CHECK();
+    return 0;
+}
+
+int rigid_move_mesh(void* verts_dev, size_t n, const RigidF& C, cudaStream_t s)
+{
+    if (!n) return 0;
+    map_rigid_mesh_kernel<<<grid_for(n), MAP_THREADS, 0, s>>>((kt_mesh_vertex*)verts_dev, n, C);
     KT_LAUNCH_CHECK();
     return 0;
 }

@@ -17,7 +17,7 @@
 // Design: the work runs over the OWNER grid [minX, min(maxX + 1, V)) x ... in fixed tiles of MESH_TILE consecutive voxels (logical
 // order), so block order is output order.  Count (per-tile vertex / triangle totals) -> CUB exclusive scan of the tile totals ->
 // vertex pass (block scan inside the tile; each vertex also writes its key 3 * owner + axis, ascending by construction) -> triangle
-// pass (keys of a cell's edges found by binary search in the key array).  No atomics, so the output does not depend on the launch;
+// pass (keys of a cell's edges found by binary search in the key array; optionally each triangle's cell as its owner-grid index).  No atomics, so the output does not depend on the launch;
 // scratch is 32 B per tile + 8 B per vertex + CUB's temporary storage.  Every pass re-derives a voxel's 3x3x3 neighbourhood from
 // the volume (L1 / L2 resident) instead of storing per-cell flags.
 #include "kt_ops.h"
@@ -213,7 +213,8 @@ __device__ __forceinline__ unsigned int find_vertex(const unsigned long long* ke
 }
 
 __global__ void __launch_bounds__(MESH_THREADS)
-mesh_triangle_kernel(const MeshParams p, const unsigned long long* toff, const unsigned long long* keys, unsigned long long n_verts, uint32_t* tris)
+mesh_triangle_kernel(const MeshParams p, const unsigned long long* toff, const unsigned long long* keys, unsigned long long n_verts, uint32_t* tris,
+                     unsigned long long* cells)
 {
     typedef cub::BlockScan<int, MESH_THREADS> Scan;
     __shared__ typename Scan::TempStorage tmp;
@@ -227,6 +228,7 @@ mesh_triangle_kernel(const MeshParams p, const unsigned long long* toff, const u
         int off, agg;
         Scan(tmp).ExclusiveSum(nt, off, agg);
         uint32_t* o = tris + 3 * (base + (unsigned long long)off);
+        if (cells) for (int k = 0; k < nt; ++k) cells[base + (unsigned long long)off + k] = (unsigned long long)idx;
         for (int k = 0; k < 3 * nt; ++k) {
             const int e = kt_mc_tris[v.mc_case][k];
             const int a = e >> 2, j = e & 3;
@@ -237,6 +239,18 @@ mesh_triangle_kernel(const MeshParams p, const unsigned long long* toff, const u
         }
         base += (unsigned long long)agg;
         __syncthreads();
+    }
+}
+
+// the global form of n local keys (see mesh_key_global): edges = vertex keys (3 * owner + axis), else triangle cells (owner)
+__global__ void __launch_bounds__(MESH_THREADS)
+mesh_global_keys_kernel(const MeshKeyFrame f, const unsigned long long* keys, unsigned long long n, bool edges, int4* out)
+{
+    for (unsigned long long i = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (unsigned long long)gridDim.x * blockDim.x) {
+        const unsigned long long k = keys[i];
+        int g[4];
+        mesh_key_global(f, edges ? k / 3 : k, edges ? (int)(k % 3) : 0, g);
+        out[i] = make_int4(g[0], g[1], g[2], g[3]);
     }
 }
 
@@ -286,17 +300,36 @@ int mesh_count(const MeshArgs& a, MeshWorkspace* ws, size_t* n_verts, size_t* n_
     return 0;
 }
 
-int mesh_emit(const MeshArgs& a, MeshWorkspace* ws, size_t n_verts, void* verts, uint32_t* tris, cudaStream_t s)
+MeshKeyFrame mesh_key_frame(const MeshArgs& a)
+{
+    MeshKeyFrame f;
+    f.min[0] = a.minX; f.min[1] = a.minY; f.min[2] = a.minZ;
+    f.ex = std::min(a.maxX + 1, a.vol) - a.minX; f.ey = std::min(a.maxY + 1, a.vol) - a.minY;
+    f.real_wrap[0] = a.real_wrap.x; f.real_wrap[1] = a.real_wrap.y; f.real_wrap[2] = a.real_wrap.z;
+    return f;
+}
+
+int mesh_emit(const MeshArgs& a, MeshWorkspace* ws, size_t n_verts, void* verts, uint32_t* tris, cudaStream_t s, unsigned long long* vkeys,
+              unsigned long long* tcells)
 {
     const MeshParams p = make_params(a);
     if (p.total == 0 || n_verts == 0) return 0;
     if (n_verts > 0xffffffffull) { set_error("mesh: %zu vertices do not fit 32-bit indices", n_verts); return KT_ERR_CAPACITY; }
     const long long nb = (p.total + MESH_TILE - 1) / MESH_TILE;
-    int r = ws->keys.grow(n_verts, with_slack(n_verts), "mesh vertex keys"); if (r) return r;
+    if (!vkeys) { int r = ws->keys.grow(n_verts, with_slack(n_verts), "mesh vertex keys"); if (r) return r; vkeys = ws->keys.get(); }
     const unsigned long long* vo = ws->counts.get() + 2 * (nb + 1); const unsigned long long* to = vo + (nb + 1);
-    mesh_vertex_kernel<<<(unsigned int)nb, MESH_THREADS, 0, s>>>(p, vo, (uint4*)verts, ws->keys.get());
+    mesh_vertex_kernel<<<(unsigned int)nb, MESH_THREADS, 0, s>>>(p, vo, (uint4*)verts, vkeys);
     KT_LAUNCH_CHECK();
-    mesh_triangle_kernel<<<(unsigned int)nb, MESH_THREADS, 0, s>>>(p, to, ws->keys.get(), n_verts, tris);
+    mesh_triangle_kernel<<<(unsigned int)nb, MESH_THREADS, 0, s>>>(p, to, vkeys, n_verts, tris, tcells);
+    KT_LAUNCH_CHECK();
+    return 0;
+}
+
+int mesh_global_keys(const MeshArgs& a, const unsigned long long* keys, size_t n, bool edges, int32_t* out, cudaStream_t s)
+{
+    if (!n) return 0;
+    const size_t b = (n + MESH_THREADS - 1) / MESH_THREADS, cap = (size_t)device_info().sm_count * 16;
+    mesh_global_keys_kernel<<<(unsigned int)std::min(b, cap), MESH_THREADS, 0, s>>>(mesh_key_frame(a), keys, n, edges, (int4*)out);
     KT_LAUNCH_CHECK();
     return 0;
 }

@@ -6,6 +6,7 @@
 
 struct kt_deform_report;
 struct kt_pgo_report;
+struct kt_weld_report;
 
 namespace kt {
 
@@ -185,8 +186,25 @@ struct MeshWorkspace {
 };
 // count + scan, then one read-back (synchronises s): the mesh's vertex and triangle counts
 int mesh_count(const MeshArgs& a, MeshWorkspace* ws, size_t* n_verts, size_t* n_tris, cudaStream_t s);
-// after mesh_count with the same arguments: writes n_verts 32-byte kt_mesh_vertex records and the triangles (3 x uint32 each); asynchronous
-int mesh_emit(const MeshArgs& a, MeshWorkspace* ws, size_t n_verts, void* verts, uint32_t* tris, cudaStream_t s);
+// after mesh_count with the same arguments: writes n_verts 32-byte kt_mesh_vertex records and the triangles (3 x uint32 each); asynchronous.
+// vkeys (may be null: the workspace's): receives every vertex's local key 3 * owner + axis; tcells (may be null): every triangle's cell
+// as the owner-grid index of its lower corner.  Neither changes the vertices or triangles.
+int mesh_emit(const MeshArgs& a, MeshWorkspace* ws, size_t n_verts, void* verts, uint32_t* tris, cudaStream_t s, unsigned long long* vkeys = nullptr,
+              unsigned long long* tcells = nullptr);
+// What turns a box's local keys into global voxels: the owner grid's origin and x / y extents, and the box's real_wrap.
+struct MeshKeyFrame { int min[3]; int ex, ey; int real_wrap[3]; };
+MeshKeyFrame mesh_key_frame(const MeshArgs& a);
+// owner-grid index -> (gx, gy, gz, axis): the logical voxel plus real_wrap, the world voxel index the positions are computed from
+__host__ __device__ inline void mesh_key_global(const MeshKeyFrame& f, unsigned long long owner, int axis, int32_t* g)
+{
+    const unsigned long long r = owner / (unsigned long long)f.ex;
+    g[0] = f.min[0] + (int)(owner % (unsigned long long)f.ex) + f.real_wrap[0];
+    g[1] = f.min[1] + (int)(r % (unsigned long long)f.ey) + f.real_wrap[1];
+    g[2] = f.min[2] + (int)(r / (unsigned long long)f.ey) + f.real_wrap[2];
+    g[3] = axis;
+}
+// n local keys -> n int32 x 4 global ones (edges: vertex keys, else triangle cells); asynchronous
+int mesh_global_keys(const MeshArgs& a, const unsigned long long* keys, size_t n, bool edges, int32_t* out, cudaStream_t s);
 // ---- embedded deformation graph (kt_deform.cu, host logic in kt_deform.hpp) ----
 // Node positions: float n x 3 (device), node times ascending.  kind: 0 kt_point_xyzrgbnormal, 1 kt_mesh_vertex, 2 packed float xyz.
 // Writes 4 node ids (int32, ascending) and 4 FP64 weights per point; asynchronous.
@@ -240,6 +258,14 @@ int voxel_grid(const void* points_dev, size_t n, int kind, float leaf, void* out
 struct RigidF { float R[9]; float t[3]; };       // row-major rotation and translation
 // x' = R x + t and n' = R n of n kt_point_xyzrgbnormal records in place, FP32 without contraction; asynchronous
 int rigid_move(void* points_dev, size_t n, const RigidF& C, cudaStream_t s);
+// the same move of n kt_mesh_vertex records in place
+int rigid_move_mesh(void* verts_dev, size_t n, const RigidF& C, cudaStream_t s);
+// ---- mesh weld (kt_weld.cu): n_meshes keyed meshes concatenated -> one mesh, every global cell and edge once; see the file header ----
+// voff / toff: n_meshes + 1 host offsets into the vertices / triangles.  rep: every field but upload_ms / download_ms.  Scratch
+// allocated and freed per call; synchronises s.
+int weld_meshes(const void* verts, const int32_t* vert_edges, const size_t* voff, const uint32_t* tris, const int32_t* tri_cells, const size_t* toff,
+                int n_meshes, void* out_verts, size_t max_verts, uint32_t* out_tris, size_t max_tris, size_t* n_verts, size_t* n_tris,
+                kt_weld_report* rep, cudaStream_t s);
 // cross-GPU barrier: every rank writes `epoch` into slot [rank] of every peer's flag array, then waits until all slots of its own
 // array reach `epoch` (bounded spin: returns through *error_dev != 0 instead of hanging the GPU if a peer never arrives)
 int xgpu_barrier(unsigned int* const* peer_flags_dev /* [world] device array of pointers */, unsigned int* my_flags, int rank, int world,

@@ -90,6 +90,7 @@ static Mat33 to_mat33(const float* m) { Mat33 r; r.r0 = make_float3(m[0], m[1], 
 // processFrame (KintinuousTracker.cpp:1166, containers/device_memory.cpp:146-157).
 struct SliceRec { int dimension; kt_point_xyzrgb* points; size_t count; kt_point_xyzrgbnormal* processed; size_t processed_count; bool has_processed;
                   kt_mesh_vertex* mesh_verts; uint32_t* mesh_tris; size_t mesh_nv, mesh_nt; bool has_mesh;
+                  unsigned long long* mesh_vkeys; unsigned long long* mesh_tcells; MeshKeyFrame mesh_frame;    // local keys: kt_get_slice_mesh_keys
                   Event ready; float camera_t[3]; float camera_R[9]; uint64_t utime; };
 
 // Pinned host memory handed out in slabs (one allocation per 64 MB, not per slice); kt_reset rewinds it, the slabs live as long as it.
@@ -208,6 +209,7 @@ struct kt_ctx {
     // marching cubes of every slice's box before it is cleared (kt_mesh.cu); buffers grow at a shift, downloaded with the slice
     int slice_meshing, mesh_weight_cull; MeshWorkspace mesh_ws; DeviceBuffer<kt_mesh_vertex> mesh_verts; DeviceBuffer<uint32_t> mesh_tris;
     size_t mesh_nv, mesh_nt;
+    DeviceBuffer<unsigned long long> mesh_vkeys, mesh_tcells; MeshKeyFrame mesh_frame;     // the slice mesh's local keys (mesh_emit) and their frame
     // the map as deformed by the last kt_deform_map (kt_deform.cu): one record per slice recorded before that call, in its own pinned
     // arena, or the slice's own buffers when the call left the map unchanged
     struct Deformed { kt_point_xyzrgbnormal* processed; kt_mesh_vertex* mesh_verts; };
@@ -281,7 +283,8 @@ int fetch_cloud(kt_ctx* c, const int* vWrapCopy, const int* lo, const int* hi)  
 // Marching cubes over the box [lo, hi) that fetch_cloud has just extracted, on the tracker stream and before the box is cleared, into
 // the context's mesh buffers (grown here: the count is read back first, once).  MeshGenerator::calculateMesh (MeshGenerator.cpp:193-227)
 // on the device, by a different algorithm (kt_mesh.cu).
-int mesh_box(kt_ctx* c, const int* vWrapCopy, const int* lo, const int* hi)
+// keyed: a slice mesh, whose local vertex keys and triangle cells go to the context's key buffers as well (no extra launch).
+int mesh_box(kt_ctx* c, const int* vWrapCopy, const int* lo, const int* hi, bool keyed)
 {
     // the previous slice's asynchronous download may still be reading the mesh buffers
     if (c->cloud_busy) { KT_CUDA(cudaStreamWaitEvent(c->stream, c->ev_cloud_free, 0)); c->cloud_busy = false; }
@@ -291,13 +294,18 @@ int mesh_box(kt_ctx* c, const int* vWrapCopy, const int* lo, const int* hi)
     a.minX = lo[0]; a.maxX = hi[0]; a.minY = lo[1]; a.maxY = hi[1]; a.minZ = lo[2]; a.maxZ = hi[2]; a.weight_cull = c->mesh_weight_cull;
     size_t nv = 0, nt = 0;
     int r = mesh_count(a, &c->mesh_ws, &nv, &nt, c->stream); if (r) return r;
-    if (nv > c->mesh_verts.capacity() || 3 * nt > c->mesh_tris.capacity()) {
+    if (nv > c->mesh_verts.capacity() || 3 * nt > c->mesh_tris.capacity() || (keyed && (nv > c->mesh_vkeys.capacity() || nt > c->mesh_tcells.capacity()))) {
         KT_CUDA(cudaStreamSynchronize(c->stream_slices));
         if ((r = c->mesh_verts.grow(nv, nv + nv / 4 + 1024, "slice mesh vertices")) ||
             (r = c->mesh_tris.grow(3 * nt, 3 * (nt + nt / 4 + 1024), "slice mesh triangles"))) return r;
+        if (keyed && ((r = c->mesh_vkeys.grow(nv, nv + nv / 4 + 1024, "slice mesh vertex keys")) ||
+                      (r = c->mesh_tcells.grow(nt, nt + nt / 4 + 1024, "slice mesh triangle cells")))) return r;
     }
-    r = mesh_emit(a, &c->mesh_ws, nv, c->mesh_verts.get(), c->mesh_tris.get(), c->stream); if (r) return r;
+    r = mesh_emit(a, &c->mesh_ws, nv, c->mesh_verts.get(), c->mesh_tris.get(), c->stream, keyed ? c->mesh_vkeys.get() : nullptr,
+                  keyed ? c->mesh_tcells.get() : nullptr);
+    if (r) return r;
     c->mesh_nv = nv; c->mesh_nt = nt;
+    if (keyed) c->mesh_frame = mesh_key_frame(a);
     return 0;
 }
 
@@ -308,7 +316,7 @@ int mesh_box(kt_ctx* c, const int* vWrapCopy, const int* lo, const int* hi)
 int push_slice(kt_ctx* c, int dimension)
 {
     SliceRec s; s.dimension = dimension; s.points = 0; s.count = c->cloud_count; s.processed = 0; s.processed_count = 0; s.has_processed = false;
-    s.has_mesh = c->slice_meshing != 0; s.mesh_verts = 0; s.mesh_tris = 0;
+    s.has_mesh = c->slice_meshing != 0; s.mesh_verts = 0; s.mesh_tris = 0; s.mesh_vkeys = 0; s.mesh_tcells = 0; s.mesh_frame = c->mesh_frame;
     s.mesh_nv = s.has_mesh ? c->mesh_nv : 0; s.mesh_nt = s.has_mesh ? c->mesh_nt : 0;
     c->proc_count = 0;
     if (c->slice_processing && c->cloud_count) {
@@ -323,7 +331,10 @@ int push_slice(kt_ctx* c, int dimension)
         if (c->proc_count) s.processed = (kt_point_xyzrgbnormal*)c->slice_arena.alloc(c->proc_count * sizeof(kt_point_xyzrgbnormal));
         if (s.mesh_nv) s.mesh_verts = (kt_mesh_vertex*)c->slice_arena.alloc(s.mesh_nv * sizeof(kt_mesh_vertex));
         if (s.mesh_nt) s.mesh_tris = (uint32_t*)c->slice_arena.alloc(s.mesh_nt * 3 * sizeof(uint32_t));
-        if ((c->cloud_count && !s.points) || (c->proc_count && !s.processed) || (s.mesh_nv && !s.mesh_verts) || (s.mesh_nt && !s.mesh_tris)) {
+        if (s.mesh_nv) s.mesh_vkeys = (unsigned long long*)c->slice_arena.alloc(s.mesh_nv * sizeof(unsigned long long));
+        if (s.mesh_nt) s.mesh_tcells = (unsigned long long*)c->slice_arena.alloc(s.mesh_nt * sizeof(unsigned long long));
+        if ((c->cloud_count && !s.points) || (c->proc_count && !s.processed) || (s.mesh_nv && (!s.mesh_verts || !s.mesh_vkeys)) ||
+            (s.mesh_nt && (!s.mesh_tris || !s.mesh_tcells))) {
             set_error("pinned host memory for a slice of %zu points", c->cloud_count); return KT_ERR_CUDA;
         }
         int r = make_event(&s.ready, cudaEventDisableTiming, "slice download"); if (r) return r;
@@ -333,6 +344,8 @@ int push_slice(kt_ctx* c, int dimension)
         if (c->proc_count) KT_CUDA(cudaMemcpyAsync(s.processed, c->proc.get(), c->proc_count * sizeof(kt_point_xyzrgbnormal), cudaMemcpyDeviceToHost, c->stream_slices));
         if (s.mesh_nv) KT_CUDA(cudaMemcpyAsync(s.mesh_verts, c->mesh_verts.get(), s.mesh_nv * sizeof(kt_mesh_vertex), cudaMemcpyDeviceToHost, c->stream_slices));
         if (s.mesh_nt) KT_CUDA(cudaMemcpyAsync(s.mesh_tris, c->mesh_tris.get(), s.mesh_nt * 3 * sizeof(uint32_t), cudaMemcpyDeviceToHost, c->stream_slices));
+        if (s.mesh_nv) KT_CUDA(cudaMemcpyAsync(s.mesh_vkeys, c->mesh_vkeys.get(), s.mesh_nv * sizeof(unsigned long long), cudaMemcpyDeviceToHost, c->stream_slices));
+        if (s.mesh_nt) KT_CUDA(cudaMemcpyAsync(s.mesh_tcells, c->mesh_tcells.get(), s.mesh_nt * sizeof(unsigned long long), cudaMemcpyDeviceToHost, c->stream_slices));
         KT_CUDA(cudaEventRecord(s.ready.get(), c->stream_slices));
         KT_CUDA(cudaEventRecord(c->ev_cloud_free, c->stream_slices));
         c->cloud_busy = true;
@@ -631,7 +644,7 @@ int process_frame_device(kt_ctx* c, uint64_t utime, kt_pose* out)
         const bool cycled = dir != 0;
         if (cycled) {
             if ((r = fetch_cloud(c, vWrapCopy, lo, hi))) return r;
-            if (c->slice_meshing && (r = mesh_box(c, vWrapCopy, lo, hi))) return r;
+            if (c->slice_meshing && (r = mesh_box(c, vWrapCopy, lo, hi, true))) return r;
             if ((r = mg_barrier(c))) return r;                          // peers may still read my boundary plane for their extraction
             if ((r = clear_volume_shared(axis, dir < 0 ? 1 : 0, c->vv, V, c->voxelWrap[axis], c->voxelWrap[axis] + n, c->stream))) return r;
         }
@@ -957,7 +970,7 @@ int kt_finalise(kt_ctx* c)                                                      
     int lo[3] = {0, 0, 0}, hi[3] = {V, V, V};
     int r = fetch_cloud(c, vWrapCopy, lo, hi);
     if (r) return r;
-    if (c->slice_meshing && (r = mesh_box(c, vWrapCopy, lo, hi))) return r;
+    if (c->slice_meshing && (r = mesh_box(c, vWrapCopy, lo, hi, true))) return r;
     return push_slice(c, 7);     // CloudSlice::FINAL
 }
 
@@ -1058,6 +1071,24 @@ int kt_get_slice_mesh(kt_ctx* c, int idx, kt_mesh_vertex* verts, size_t max_vert
     return KT_OK;
 }
 
+// the expanded keys of slice s: up to max_verts vertex edges and max_tris triangle cells (4 x int32 each)
+static void slice_mesh_keys(const SliceRec& s, int32_t* vert_edges, size_t max_verts, int32_t* tri_cells, size_t max_tris)
+{
+    const size_t nv = vert_edges ? std::min(max_verts, s.mesh_nv) : 0, nt = tri_cells ? std::min(max_tris, s.mesh_nt) : 0;
+    for (size_t i = 0; i < nv; ++i) mesh_key_global(s.mesh_frame, s.mesh_vkeys[i] / 3, (int)(s.mesh_vkeys[i] % 3), vert_edges + 4 * i);
+    for (size_t i = 0; i < nt; ++i) mesh_key_global(s.mesh_frame, s.mesh_tcells[i], 0, tri_cells + 4 * i);
+}
+
+int kt_get_slice_mesh_keys(kt_ctx* c, int idx, int32_t* vert_edges, size_t max_verts, int32_t* tri_cells, size_t max_tris)
+{
+    if (!c || idx < 0 || idx >= (int)c->slices.size()) { set_error("kt_get_slice_mesh_keys: bad index"); return KT_ERR_INVALID; }
+    const SliceRec& s = c->slices[idx];
+    if (!s.has_mesh) { set_error("kt_get_slice_mesh_keys: slice %d was recorded with meshing off (kt_set_slice_meshing)", idx); return KT_ERR_STATE; }
+    if (s.mesh_nv) KT_CUDA(cudaEventSynchronize(s.ready.get()));
+    slice_mesh_keys(s, vert_edges, max_verts, tri_cells, max_tris);
+    return KT_OK;
+}
+
 int kt_get_live_mesh(kt_ctx* c, kt_mesh_vertex* verts, size_t max_verts, uint32_t* tris, size_t max_tris, size_t* n_verts, size_t* n_tris)
 {
     if (!c) return KT_ERR_INVALID;
@@ -1066,7 +1097,7 @@ int kt_get_live_mesh(kt_ctx* c, kt_mesh_vertex* verts, size_t max_verts, uint32_
     int vWrapCopy[3]; vwrap_copy(c, vWrapCopy);
     const int V = c->cfg.vol;
     int lo[3] = {0, 0, 0}, hi[3] = {V, V, V};
-    int r = mesh_box(c, vWrapCopy, lo, hi);
+    int r = mesh_box(c, vWrapCopy, lo, hi, false);
     if (r) return r;
     if (n_verts) *n_verts = c->mesh_nv;
     if (n_tris) *n_tris = c->mesh_nt;
@@ -1077,12 +1108,14 @@ int kt_get_live_mesh(kt_ctx* c, kt_mesh_vertex* verts, size_t max_verts, uint32_
     return KT_OK;
 }
 
-// The meshes of the first n_slices slices as one binary PLY; with `deformed`, the vertices of the last kt_deform_map
-static int save_mesh_ply(kt_ctx* c, const char* path, size_t n_slices, bool deformed, const char* who)
+// A mesh as parts written back to back: every part's vertices, then every part's triangles with the part's vertices' offset added
+struct PlyPart { const kt_mesh_vertex* v; size_t nv; const uint32_t* t; size_t nt; };
+
+// One binary little-endian PLY (vertex: float x y z nx ny nz, uchar red green blue; face: list uchar int vertex_indices)
+static int write_mesh_ply(const char* path, const std::vector<PlyPart>& parts, const char* who)
 {
-    size_t nv = 0, nt = 0; bool any = false;
-    for (size_t i = 0; i < n_slices; ++i) { const auto& s = c->slices[i]; if (s.has_mesh) { any = true; nv += s.mesh_nv; nt += s.mesh_nt; } }
-    if (!any) { set_error("%s: no slice was recorded with meshing on (kt_set_slice_meshing)", who); return KT_ERR_STATE; }
+    size_t nv = 0, nt = 0;
+    for (const PlyPart& p : parts) { nv += p.nv; nt += p.nt; }
     if (nv > 0x7fffffffu) { set_error("%s: %zu vertices do not fit the PLY's int indices", who, nv); return KT_ERR_CAPACITY; }
     FILE* f = fopen(path, "wb");
     if (!f) { set_error("%s: cannot open %s", who, path); return KT_ERR_INVALID; }
@@ -1091,34 +1124,45 @@ static int save_mesh_ply(kt_ctx* c, const char* path, size_t n_slices, bool defo
                "element face %zu\nproperty list uchar int vertex_indices\nend_header\n", nv, nt);
     std::vector<unsigned char> buf;
     bool ok = true;
-    for (size_t k = 0; k < n_slices; ++k) {                        // x86 / aarch64 hosts are little-endian: records are the raw bytes
-        const auto& s = c->slices[k];
-        if (!s.has_mesh || !s.mesh_nv) continue;
-        if (cudaEventSynchronize(s.ready.get()) != cudaSuccess) { ok = false; break; }
-        const kt_mesh_vertex* mv = deformed ? c->deformed[k].mesh_verts : s.mesh_verts;
-        buf.resize(s.mesh_nv * 27);
-        for (size_t i = 0; i < s.mesh_nv; ++i) {
-            std::memcpy(&buf[i * 27], &mv[i].x, 24);
-            buf[i * 27 + 24] = mv[i].r; buf[i * 27 + 25] = mv[i].g; buf[i * 27 + 26] = mv[i].b;
+    for (const PlyPart& p : parts) {                              // x86 / aarch64 hosts are little-endian: records are the raw bytes
+        if (!p.nv) continue;
+        buf.resize(p.nv * 27);
+        for (size_t i = 0; i < p.nv; ++i) {
+            std::memcpy(&buf[i * 27], &p.v[i].x, 24);
+            buf[i * 27 + 24] = p.v[i].r; buf[i * 27 + 25] = p.v[i].g; buf[i * 27 + 26] = p.v[i].b;
         }
         ok = ok && fwrite(buf.data(), 1, buf.size(), f) == buf.size();
     }
     uint32_t base = 0;
-    for (size_t k = 0; k < n_slices; ++k) {
-        const auto& s = c->slices[k];
+    for (const PlyPart& p : parts) {
         if (!ok) break;
-        if (!s.has_mesh) continue;
-        buf.resize(s.mesh_nt * 13);
-        for (size_t t = 0; t < s.mesh_nt; ++t) {
+        buf.resize(p.nt * 13);
+        for (size_t t = 0; t < p.nt; ++t) {
             buf[t * 13] = 3;
-            for (int k = 0; k < 3; ++k) { const int32_t v = (int32_t)(s.mesh_tris[3 * t + k] + base); std::memcpy(&buf[t * 13 + 1 + 4 * k], &v, 4); }
+            for (int k = 0; k < 3; ++k) { const int32_t v = (int32_t)(p.t[3 * t + k] + base); std::memcpy(&buf[t * 13 + 1 + 4 * k], &v, 4); }
         }
         ok = ok && fwrite(buf.data(), 1, buf.size(), f) == buf.size();
-        base += (uint32_t)s.mesh_nv;
+        base += (uint32_t)p.nv;
     }
     if (fclose(f) != 0) ok = false;
     if (!ok) { set_error("%s: writing %s failed", who, path); return KT_ERR_CUDA; }
     return KT_OK;
+}
+
+// The meshes of the first n_slices slices as one binary PLY; with `deformed`, the vertices of the last kt_deform_map
+static int save_mesh_ply(kt_ctx* c, const char* path, size_t n_slices, bool deformed, const char* who)
+{
+    bool any = false;
+    for (size_t i = 0; i < n_slices; ++i) if (c->slices[i].has_mesh) any = true;
+    if (!any) { set_error("%s: no slice was recorded with meshing on (kt_set_slice_meshing)", who); return KT_ERR_STATE; }
+    std::vector<PlyPart> parts;
+    for (size_t k = 0; k < n_slices; ++k) {
+        const auto& s = c->slices[k];
+        if (!s.has_mesh) continue;
+        if (s.mesh_nv) KT_CUDA(cudaEventSynchronize(s.ready.get()));
+        parts.push_back(PlyPart{deformed ? c->deformed[k].mesh_verts : s.mesh_verts, s.mesh_nv, s.mesh_tris, s.mesh_nt});
+    }
+    return write_mesh_ply(path, parts, who);
 }
 
 int kt_save_mesh_ply(kt_ctx* c, const char* path)
@@ -1661,6 +1705,29 @@ int kt_save_deformed_mesh_ply(kt_ctx* c, const char* path)
     return save_mesh_ply(c, path, c->deformed.size(), true, "kt_save_deformed_mesh_ply");
 }
 
+// The correction slices recorded after the last deformation follow: C = P_corr(t) P_tracked(t)^-1 in FP64, the rigid inverse
+// [R^T | -R^T t], rounded to float
+static RigidF map_correction(const kt_ctx* c)
+{
+    const float* Pt = c->map_corr.tracked; const float* Pc = c->map_corr.corrected;
+    RigidF C;
+    for (int a = 0; a < 3; ++a) {
+        for (int b = 0; b < 3; ++b) {
+            double v = 0;
+            for (int k = 0; k < 3; ++k) v += (double)Pc[4 * a + k] * (double)Pt[4 * b + k];
+            C.R[3 * a + b] = (float)v;
+        }
+        double t = Pc[4 * a + 3];
+        for (int b = 0; b < 3; ++b) {
+            double v = 0;
+            for (int k = 0; k < 3; ++k) v += (double)Pc[4 * a + k] * (double)Pt[4 * b + k];
+            t -= v * (double)Pt[4 * b + 3];
+        }
+        C.t[a] = (float)t;
+    }
+    return C;
+}
+
 // The map as one cloud (kt_get_map_cloud, kt_save_map_pcd; the header describes which / dedupe).  The points go to out (up to capacity),
 // or, with `grow`, to a host vector sized to the full count.  Device work, if any, runs on the slice stream with scratch that is freed
 // before returning; nothing the tracker reads is written.
@@ -1715,26 +1782,7 @@ static int map_cloud(kt_ctx* c, int which, int dedupe, kt_point_xyzrgbnormal* ou
             off += sl.processed_count;
         }
         KT_CUDA(cudaEventRecord(ev[1], s));
-        if (n_fixed < n) {
-            // C = P_corr(t) P_tracked(t)^-1 in FP64, the rigid inverse [R^T | -R^T t], rounded to float
-            const float* Pt = c->map_corr.tracked; const float* Pc = c->map_corr.corrected;
-            RigidF C;
-            for (int a = 0; a < 3; ++a) {
-                for (int b = 0; b < 3; ++b) {
-                    double v = 0;
-                    for (int k = 0; k < 3; ++k) v += (double)Pc[4 * a + k] * (double)Pt[4 * b + k];
-                    C.R[3 * a + b] = (float)v;
-                }
-                double t = Pc[4 * a + 3];
-                for (int b = 0; b < 3; ++b) {
-                    double v = 0;
-                    for (int k = 0; k < 3; ++k) v += (double)Pc[4 * a + k] * (double)Pt[4 * b + k];
-                    t -= v * (double)Pt[4 * b + 3];
-                }
-                C.t[a] = (float)t;
-            }
-            int r = rigid_move((kt_point_xyzrgbnormal*)d_in + n_fixed, n - n_fixed, C, s); if (r) return r;
-        }
+        if (n_fixed < n) { int r = rigid_move((kt_point_xyzrgbnormal*)d_in + n_fixed, n - n_fixed, map_correction(c), s); if (r) return r; }
         size_t m = n;
         float ms2[2] = {0.f, 0.f};
         if (dedupe) { int r = voxel_grid(d_in, n, 1, c->voxel, d_out, n, &m, &R.pcl_would_skip, ms2, s); if (r) return r; }
@@ -1789,6 +1837,123 @@ int kt_save_map_pcd(kt_ctx* c, const char* path, int which, int dedupe, kt_map_r
     if (fclose(f) != 0) ok = false;
     if (!ok) { set_error("kt_save_map_pcd: writing %s failed", path); return KT_ERR_CUDA; }
     return KT_OK;
+}
+
+// The map as one mesh (kt_get_map_mesh, kt_save_map_ply; the header describes which / weld).  The mesh goes to verts / tris (up to the
+// capacities), or, with gv / gt, to host vectors sized to the full counts.  Device work, if any, runs on the slice stream with scratch
+// that is freed before returning; nothing the tracker reads is written.
+static int map_mesh(kt_ctx* c, int which, bool weld, kt_mesh_vertex* verts, size_t max_verts, uint32_t* tris, size_t max_tris,
+                    std::vector<kt_mesh_vertex>* gv, std::vector<uint32_t>* gt, size_t* n_verts, size_t* n_tris, kt_weld_report* report, const char* who)
+{
+    kt_weld_report R; std::memset(&R, 0, sizeof(R));
+    if (report) *report = R;
+    *n_verts = 0; *n_tris = 0;
+    if (which != 0 && which != 1) { set_error("%s: which must be 0 (recorded map) or 1 (corrected map)", who); return KT_ERR_INVALID; }
+    if (c->world > 1) { set_error("%s: a volume shared by %d GPUs cannot be meshed", who, c->world); return KT_ERR_INVALID; }
+    KT_CUDA(cudaSetDevice(c->cfg.device));
+    if (c->stream_slices) KT_CUDA(cudaStreamSynchronize(c->stream_slices));           // every slice has landed in its pinned buffers
+    // slices [0, covered) come from the deformed copies; with which = 1 the later ones are moved rigidly and follow them
+    const size_t covered = which == 1 ? c->deformed.size() : c->slices.size();
+    std::vector<size_t> ids, voff(1, 0), toff(1, 0);
+    size_t n_fixed = 0;
+    for (size_t i = 0; i < c->slices.size(); ++i) {
+        const SliceRec& s = c->slices[i];
+        if (!s.has_mesh) continue;
+        ids.push_back(i); voff.push_back(voff.back() + s.mesh_nv); toff.push_back(toff.back() + s.mesh_nt);
+        if (i < covered) n_fixed += s.mesh_nv; else ++R.moved_meshes;
+    }
+    if (ids.empty()) { set_error("%s: no slice was recorded with meshing on (kt_set_slice_meshing)", who); return KT_ERR_STATE; }
+    if (which == 1 && c->deformed.empty()) { set_error("%s: no kt_deform_map / kt_close_loop has deformed the map since the last reset", who); return KT_ERR_STATE; }
+    const size_t nv = voff.back(), nt = toff.back(), rec = sizeof(kt_mesh_vertex);
+    R.meshes = (int)ids.size(); R.input_verts = nv; R.input_tris = nt;
+    if (nv > 0xffffffffull) { set_error("%s: %zu vertices do not fit 32-bit indices", who, nv); return KT_ERR_CAPACITY; }
+    auto src = [&](size_t i) -> const kt_mesh_vertex* { return which == 1 && i < covered ? c->deformed[i].mesh_verts : c->slices[i].mesh_verts; };
+    auto sized = [&](size_t ov, size_t ot) {
+        R.output_verts = ov; R.output_tris = ot;
+        if (gv) { gv->resize(ov); gt->resize(3 * ot); verts = gv->data(); tris = gt->data(); max_verts = ov; max_tris = ot; }
+        if (!verts) max_verts = 0;
+        if (!tris) max_tris = 0;
+    };
+    auto concat_tris = [&]() {                                       // the slices' triangles, indices offset by the vertices before them
+        for (size_t k = 0; k < ids.size() && toff[k] < max_tris; ++k) {
+            const SliceRec& s = c->slices[ids[k]];
+            const size_t m = std::min(s.mesh_nt, max_tris - toff[k]);
+            for (size_t j = 0; j < 3 * m; ++j) tris[3 * toff[k] + j] = s.mesh_tris[j] + (uint32_t)voff[k];
+        }
+    };
+    if (!weld && n_fixed == nv) {                                    // a concatenation of pinned host buffers
+        sized(nv, nt);
+        for (size_t k = 0; k < ids.size() && voff[k] < max_verts; ++k)
+            std::memcpy(verts + voff[k], src(ids[k]), std::min(voff[k + 1], max_verts) * rec - voff[k] * rec);
+        concat_tris();
+    } else {
+        cudaStream_t s = c->stream_slices;
+        Allocations mem(s);
+        cudaEvent_t ev[4];
+        for (int e = 0; e < 4; ++e) if (mem.event(&ev[e], cudaEventDefault, who)) return KT_ERR_CUDA;
+        kt_mesh_vertex* d_v = 0; kt_mesh_vertex* d_ov = 0; int32_t* d_e = 0; int32_t* d_c = 0; uint32_t* d_t = 0; uint32_t* d_ot = 0;
+        if (mem.device(&d_v, std::max(nv, (size_t)1), who) ||
+            (weld && (mem.device(&d_e, 4 * std::max(nv, (size_t)1), who) || mem.device(&d_c, 4 * std::max(nt, (size_t)1), who) ||
+                      mem.device(&d_t, 3 * std::max(nt, (size_t)1), who) || mem.device(&d_ov, std::max(nv, (size_t)1), who) ||
+                      mem.device(&d_ot, 3 * std::max(nt, (size_t)1), who)))) return KT_ERR_CUDA;
+        std::vector<int32_t> edges, cells;
+        if (weld) {                                                  // the keys' global form, expanded on the host from the compact local keys
+            edges.resize(4 * nv); cells.resize(4 * nt);
+            for (size_t k = 0; k < ids.size(); ++k) {
+                const SliceRec& sl = c->slices[ids[k]];
+                slice_mesh_keys(sl, edges.data() + 4 * voff[k], sl.mesh_nv, cells.data() + 4 * toff[k], sl.mesh_nt);
+            }
+        }
+        KT_CUDA(cudaEventRecord(ev[0], s));
+        for (size_t k = 0; k < ids.size(); ++k) {
+            const SliceRec& sl = c->slices[ids[k]];
+            if (sl.mesh_nv) KT_CUDA(cudaMemcpyAsync(d_v + voff[k], src(ids[k]), sl.mesh_nv * rec, cudaMemcpyHostToDevice, s));
+            if (weld && sl.mesh_nt) KT_CUDA(cudaMemcpyAsync(d_t + 3 * toff[k], sl.mesh_tris, sl.mesh_nt * 3 * sizeof(uint32_t), cudaMemcpyHostToDevice, s));
+        }
+        if (weld) {
+            if (nv) KT_CUDA(cudaMemcpyAsync(d_e, edges.data(), edges.size() * sizeof(int32_t), cudaMemcpyHostToDevice, s));
+            if (nt) KT_CUDA(cudaMemcpyAsync(d_c, cells.data(), cells.size() * sizeof(int32_t), cudaMemcpyHostToDevice, s));
+        }
+        KT_CUDA(cudaEventRecord(ev[1], s));
+        if (n_fixed < nv) { int r = rigid_move_mesh(d_v + n_fixed, nv - n_fixed, map_correction(c), s); if (r) return r; }
+        size_t ov = nv, ot = nt;
+        if (weld) {
+            kt_weld_report W;
+            int r = weld_meshes(d_v, d_e, voff.data(), d_t, d_c, toff.data(), (int)ids.size(), d_ov, nv, d_ot, nt, &ov, &ot, &W, s); if (r) return r;
+            R.repeated_cells = W.repeated_cells; R.dropped_triangles = W.dropped_triangles; R.merged_vertices = W.merged_vertices;
+            R.sort_ms = W.sort_ms; R.weld_ms = W.weld_ms;
+        }
+        sized(ov, ot);
+        KT_CUDA(cudaEventRecord(ev[2], s));
+        const size_t kv = std::min(ov, max_verts), kt = std::min(ot, max_tris);
+        if (kv) KT_CUDA(cudaMemcpyAsync(verts, weld ? d_ov : d_v, kv * rec, cudaMemcpyDeviceToHost, s));
+        if (weld && kt) KT_CUDA(cudaMemcpyAsync(tris, d_ot, kt * 3 * sizeof(uint32_t), cudaMemcpyDeviceToHost, s));
+        KT_CUDA(cudaEventRecord(ev[3], s));
+        if (!weld) concat_tris();
+        KT_CUDA(cudaStreamSynchronize(s));
+        KT_CUDA(cudaEventElapsedTime(&R.upload_ms, ev[0], ev[1]));
+        KT_CUDA(cudaEventElapsedTime(&R.download_ms, ev[2], ev[3]));
+        KT_CUDA(cudaEventElapsedTime(&R.total_ms, ev[0], ev[3]));
+    }
+    *n_verts = R.output_verts; *n_tris = R.output_tris;
+    if (report) *report = R;
+    return KT_OK;
+}
+
+int kt_get_map_mesh(kt_ctx* c, int which, int weld, kt_mesh_vertex* verts, size_t max_verts, uint32_t* tris, size_t max_tris, size_t* n_verts,
+                    size_t* n_tris, kt_weld_report* report)
+{
+    if (!c || !n_verts || !n_tris) { set_error("kt_get_map_mesh: bad argument"); return KT_ERR_INVALID; }
+    return map_mesh(c, which, weld != 0, verts, verts ? max_verts : 0, tris, tris ? max_tris : 0, 0, 0, n_verts, n_tris, report, "kt_get_map_mesh");
+}
+
+int kt_save_map_ply(kt_ctx* c, const char* path, int which, int weld, kt_weld_report* report)
+{
+    if (!c || !path) { set_error("kt_save_map_ply: bad argument"); return KT_ERR_INVALID; }
+    std::vector<kt_mesh_vertex> v; std::vector<uint32_t> t;
+    size_t nv = 0, nt = 0;
+    int r = map_mesh(c, which, weld != 0, 0, 0, 0, 0, &v, &t, &nv, &nt, report, "kt_save_map_ply"); if (r) return r;
+    return write_mesh_ply(path, std::vector<PlyPart>(1, PlyPart{v.data(), nv, t.data(), nt}), "kt_save_map_ply");
 }
 
 int kt_get_slice_info(kt_ctx* c, int idx, kt_slice_info* info)
