@@ -53,6 +53,14 @@ int ensure_scratch()
     o.mem = std::move(m); o.state = state; o.partials = partials; o.ipartials = ipartials; o.counter = counter; o.host_state = host_state;
     return 0;
 }
+// The volume operators' one requirement on vol (include/kintinuous_b200.h): a positive multiple of 8.  The y / z clear stores 16-byte
+// words along a row and init_volume fills whole 16-byte words, so any other side would misalign those stores or leave voxels unwritten.
+int check_vol(const char* who, int vol)
+{
+    if (vol <= 0 || vol % 8 != 0) { set_error("%s: vol %d is not a positive multiple of 8", who, vol); return KT_ERR_INVALID; }
+    return KT_OK;
+}
+
 int ensure_ztable(int vol)
 {
     const size_t n = vol > 0 ? (size_t)2 * vol : 0;
@@ -132,8 +140,9 @@ int kt_op_integrate(const uint16_t* depth_raw, int rows, int cols, const float* 
                     const float* Rinv, const float* t, float trunc, int16_t* tsdf, uint8_t* color, int vol,
                     const int* wrap, const uint8_t* rgb, const float* nmap_curr, int angle_color, float* depth_scaled, void* s)
 {
+    int r = check_vol("kt_op_integrate", vol); if (r) return r;
     KT_OPS_LOCK();
-    int r = ensure_ztable(vol); if (r) return r;
+    r = ensure_ztable(vol); if (r) return r;
     r = scale_depth(depth_raw, depth_scaled, rows, cols, intr4(k), angle_color != 0, st(s)); if (r) return r;
     IntegrateArgs a; a.cw = 0; a.rgbf = 0; a.reset_words = 0; a.reset_count = 0; a.reset_stride = 1;
     a.depth_scaled = depth_scaled; a.rows = rows; a.cols = cols; a.k = intr4(k); a.volume_size = make_float3(vs[0], vs[1], vs[2]);
@@ -149,7 +158,10 @@ int kt_op_raycast(const float* k, const float* R, const float* t, float trunc, c
                   const int16_t* tsdf, int vol, float* vmap, float* nmap, int rows, int cols,
                   const int* wrap, uint8_t* vmap_color, const uint8_t* color, void* s)
 {
-    RaycastArgs a;
+    // a cell size the ray cast cannot divide by is wrong whatever the side, so it is named first (a side <= 0 has no cell: check_vol)
+    if (vol > 0) { if (int r = check_cell_size(make_float3(vs[0], vs[1], vs[2]), vol)) return r; }
+    if (int r = check_vol("kt_op_raycast", vol)) return r;
+    RaycastArgs a = {};          // multi = 0 (one volume) and no field left for raycast() to read uninitialised
     a.k = intr4(k); a.R = mat33(R); a.t = make_float3(t[0], t[1], t[2]); a.trunc = trunc; a.volume_size = make_float3(vs[0], vs[1], vs[2]);
     a.tsdf = tsdf; a.color = color; a.vol = vol; a.wrap = make_int3(wrap[0], wrap[1], wrap[2]);
     for (int l = 0; l < LEVELS; ++l) { a.vmap[l] = vmap; a.nmap[l] = nmap; }
@@ -163,8 +175,9 @@ int kt_op_extract_slice(const int16_t* tsdf, const float* vs, int vol, kt_point_
                         const int* wrap, const uint8_t* color, int minX, int maxX, int minY, int maxY, int minZ, int maxZ,
                         int subsample, const int* real_wrap, size_t* count, void* s)
 {
+    int r = check_vol("kt_op_extract_slice", vol); if (r) return r;
     KT_OPS_LOCK();
-    int r = ensure_scratch(); if (r) return r;
+    r = ensure_scratch(); if (r) return r;
     KT_CUDA(cudaMemsetAsync(g_ops.counter, 0, sizeof(unsigned int), st(s)));
     r = extract_slice(tsdf, make_float3(vs[0], vs[1], vs[2]), vol, out, capacity, make_int3(wrap[0], wrap[1], wrap[2]), color,
                       minX, maxX, minY, maxY, minZ, maxZ, subsample, make_int3(real_wrap[0], real_wrap[1], real_wrap[2]), g_ops.counter, st(s));
@@ -193,7 +206,8 @@ int kt_op_mesh_volume(const int16_t* tsdf, const uint8_t* color, int vol, const 
                       int minX, int maxX, int minY, int maxY, int minZ, int maxZ, int weight_cull, kt_mesh_vertex* verts, size_t max_verts,
                       uint32_t* tris, size_t max_tris, size_t* n_verts, size_t* n_tris, void* s)
 {
-    if (!tsdf || !color || !vs || !wrap || !real_wrap || !n_verts || !n_tris || vol <= 0) { set_error("kt_op_mesh_volume: bad argument"); return KT_ERR_INVALID; }
+    if (int r = check_vol("kt_op_mesh_volume", vol)) return r;
+    if (!tsdf || !color || !vs || !wrap || !real_wrap || !n_verts || !n_tris) { set_error("kt_op_mesh_volume: bad argument"); return KT_ERR_INVALID; }
     if (minX < 0 || minY < 0 || minZ < 0 || maxX > vol || maxY > vol || maxZ > vol) { set_error("kt_op_mesh_volume: box outside [0, vol]"); return KT_ERR_INVALID; }
     KT_OPS_LOCK();
     MeshArgs a;
@@ -213,7 +227,8 @@ int kt_op_mesh_volume_keyed(const int16_t* tsdf, const uint8_t* color, int vol, 
                             int minX, int maxX, int minY, int maxY, int minZ, int maxZ, int weight_cull, kt_mesh_vertex* verts, int32_t* vert_edges,
                             size_t max_verts, uint32_t* tris, int32_t* tri_cells, size_t max_tris, size_t* n_verts, size_t* n_tris, void* s)
 {
-    if (!tsdf || !color || !vs || !wrap || !real_wrap || !n_verts || !n_tris || vol <= 0) { set_error("kt_op_mesh_volume_keyed: bad argument"); return KT_ERR_INVALID; }
+    if (int r = check_vol("kt_op_mesh_volume_keyed", vol)) return r;
+    if (!tsdf || !color || !vs || !wrap || !real_wrap || !n_verts || !n_tris) { set_error("kt_op_mesh_volume_keyed: bad argument"); return KT_ERR_INVALID; }
     if (minX < 0 || minY < 0 || minZ < 0 || maxX > vol || maxY > vol || maxZ > vol) { set_error("kt_op_mesh_volume_keyed: box outside [0, vol]"); return KT_ERR_INVALID; }
     KT_OPS_LOCK();
     MeshArgs a;
@@ -291,10 +306,18 @@ int kt_op_deform_apply(const float* node_pos, const double* params, int n_nodes,
 }
 
 int kt_op_clear_volume(int axis, int back, int16_t* tsdf, uint8_t* color, int vol, int current, int delta, void* s)
-{ int r = clear_volume(axis, back, tsdf, color, vol, current, delta, st(s)); if (r) return r; KT_CUDA(cudaStreamSynchronize(st(s))); return KT_OK; }
+{
+    int r = check_vol("kt_op_clear_volume", vol); if (r) return r;
+    r = clear_volume(axis, back, tsdf, color, vol, current, delta, st(s)); if (r) return r;
+    KT_CUDA(cudaStreamSynchronize(st(s))); return KT_OK;
+}
 
 int kt_op_init_volume(int16_t* tsdf, uint8_t* color, int vol, void* s)
-{ int r = init_volume(tsdf, color, vol, st(s)); if (r) return r; KT_CUDA(cudaStreamSynchronize(st(s))); return KT_OK; }
+{
+    int r = check_vol("kt_op_init_volume", vol); if (r) return r;
+    r = init_volume(tsdf, color, vol, st(s)); if (r) return r;
+    KT_CUDA(cudaStreamSynchronize(st(s))); return KT_OK;
+}
 
 int kt_op_short_depth_to_metres(const uint16_t* src, float* dst, int rows, int cols, int cut, void* s)
 { int r = short_depth_to_metres(src, dst, rows, cols, cut, st(s)); if (r) return r; KT_CUDA(cudaStreamSynchronize(st(s))); return KT_OK; }

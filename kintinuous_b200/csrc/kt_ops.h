@@ -158,6 +158,7 @@ struct RaycastArgs {
     float* peer_vmap[MAX_GPUS][LEVELS]; float* peer_nmap[MAX_GPUS][LEVELS]; uint8_t* peer_vcol[MAX_GPUS];
 };
 int raycast(const RaycastArgs& a, cudaStream_t s);
+int check_cell_size(const float3& volume_size, int vol);      // raycast()'s refusal of a cell size it cannot divide by (-1, error set)
 int extract_slice(const int16_t* tsdf, const float3& volume_size, int vol, void* out, size_t capacity, const int3& wrap,
                   const uint8_t* color, int minX, int maxX, int minY, int maxY, int minZ, int maxZ, int subsample,
                   const int3& real_wrap, unsigned int* counter_dev, cudaStream_t s);

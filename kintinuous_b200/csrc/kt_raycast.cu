@@ -423,6 +423,14 @@ raycast_kernel(const RayParams p)
 
 } // namespace
 
+// every quotient by the cell size is a multiply by its reciprocal (rcp_approx), which equals the division only up to 2^126
+int check_cell_size(const float3& volume_size, int vol)
+{
+    const float3 cs = make_float3(volume_size.x / vol, volume_size.y / vol, volume_size.z / vol);
+    if (!(fabsf(cs.x) <= 0x1p126f && fabsf(cs.y) <= 0x1p126f && fabsf(cs.z) <= 0x1p126f)) { set_error("raycast: cell size (volume_size / vol) must be finite and at most 2^126"); return -1; }
+    return 0;
+}
+
 int raycast(const RaycastArgs& a, cudaStream_t s)
 {
     RayParams p;
@@ -432,9 +440,7 @@ int raycast(const RaycastArgs& a, cudaStream_t s)
     for (int l = 0; l < LEVELS; ++l) { p.vmap[l] = a.vmap[l]; p.nmap[l] = a.nmap[l]; }
     p.vmap_color = (uchar4*)a.vmap_color; p.rows = a.rows; p.cols = a.cols;
     p.n_levels = a.n_levels; p.z_begin = 0; p.tile_row_begin = 0; p.n_out = 1;
-    // every quotient by the cell size is a multiply by its reciprocal (rcp_approx), which equals the division only up to 2^126
-    const float3 cs = p.cell_size;
-    if (!(fabsf(cs.x) <= 0x1p126f && fabsf(cs.y) <= 0x1p126f && fabsf(cs.z) <= 0x1p126f)) { set_error("raycast: cell size (volume_size / vol) must be finite and at most 2^126"); return -1; }
+    if (int r = check_cell_size(a.volume_size, a.vol)) return r;
     // the in-tile pyramid needs every level's tile to be whole
     if (p.n_levels > 1 && ((a.cols % RC_X) != 0 || (a.rows % RC_Y) != 0)) { set_error("raycast: fused pyramid needs cols %% 16 == 0 and rows %% 8 == 0"); return -1; }
     dim3 block(RC_X, RC_Y), grid(div_up(a.cols, RC_X), div_up(a.rows, RC_Y));

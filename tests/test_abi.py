@@ -59,6 +59,30 @@ def test_config_validation(built):
     assert lib.kt_create(None, ctypes.byref(h)) != 0
 
 
+@pytest.mark.parametrize("vol", [100, 33, 4, 0, -8])
+def test_volume_operators_refuse_a_side_that_is_not_a_multiple_of_8(built, vol):
+    """Every volume operator refuses vol % 8 != 0 (and vol <= 0) with KT_ERR_INVALID before it launches anything: at V = 100 the y / z
+    clear's 16-byte row stores would be misaligned and miss each row's last 4 voxels, at V = 33 init_volume would leave the last voxel
+    unwritten.  The pointers are NULL: a call that got past the check would fail differently (or fault), so this needs no GPU."""
+    import kintinuous_b200 as kb
+    ops = kb.ops
+    eye, t3, intr, vs = np.eye(3, dtype=np.float32), np.full(3, 3.0, np.float32), np.array([132.0, 132.0, 80.0, 66.75], np.float32), [6.0] * 3
+    calls = {
+        "kt_op_init_volume": lambda: ops.init_volume(None, None, vol),
+        "kt_op_clear_volume": lambda: ops.clear_volume(1, 0, None, None, vol, 0, 14),
+        "kt_op_integrate": lambda: ops.integrate(None, 120, 160, intr, vs, eye, t3, 0.06, None, None, vol, (0, 0, 0), None, None, 1, None),
+        "kt_op_raycast": lambda: ops.raycast(intr, eye, t3, 0.06, vs, None, vol, None, None, 120, 160, (0, 0, 0), None, None),
+        "kt_op_extract_slice": lambda: ops.extract_slice(None, vs, vol, None, 10, (0, 0, 0), None, (0, 8, 0, 8, 0, 8), 1, (0, 0, 0)),
+        "kt_op_mesh_volume": lambda: ops.mesh_volume_into(None, None, vol, vs, (0, 0, 0), (0, 0, 0), (0, 8, 0, 8, 0, 8), 8, None, 0, None, 0),
+        "kt_op_mesh_volume_keyed": lambda: ops.mesh_volume_keyed_into(None, None, vol, vs, (0, 0, 0), (0, 0, 0), (0, 8, 0, 8, 0, 8), 8, None, None, 0,
+                                                                     None, None, 0),
+    }
+    for name, call in calls.items():
+        with pytest.raises(kb.KtError) as e:
+            call()
+        assert f"{name}: vol {vol} is not a positive multiple of 8" in str(e.value), (name, str(e.value))
+
+
 def test_product_never_touches_the_oracle():
     """The product path must not import, link or execute anything under oracle/."""
     pkg = os.path.join(ROOT, "kintinuous_b200")

@@ -30,6 +30,9 @@ Three statements per run, each exact or with its tolerance written here:
 
 3. SLICES, EXACT.  At each shift the slab the product hands out must equal, as a multiset of 32-byte points, what the reference's
    extractCloudSlice returns on the replayed volume for the same box (extract.cu:325-419; slab boxes from KintinuousTracker.cpp:675-831).
+
+The ICP-only run is also made at 384^3 (tests/golden/ref_baseline_384_odo0.npz, the reference compiled for VOL=384): a legal tracker
+side that is not a power of two, so the tracker's ray cast with its in-tile pyramid and its shift boxes run their non-power-of-two code.
 """
 import os
 
@@ -51,7 +54,7 @@ def rot_angle(Ra, Rb):
     return float(np.linalg.norm(w))
 
 
-def vwrap_nonneg(w):                      # KintinuousTracker::vWrapCopyUpdate (.cpp:1075-1085)
+def vwrap_nonneg(w, V=V):                 # KintinuousTracker::vWrapCopyUpdate (.cpp:1075-1085)
     return [int(x) if x >= 0 else V - ((-int(x)) % V) for x in w]
 
 
@@ -68,11 +71,17 @@ def frames26():
         return [synth.render(k) for k in range(72)]
 
 
-@pytest.mark.parametrize("odometry,nframes", [(0, 72), (2, 22), (1, 26)])
-def test_baseline_config_512_live_replay_exact(built, frames26, odometry, nframes):
+# (V, odometry, frames, shifts within the stable horizon, horizon bound): 384^3 is not a power of two -- the only run of the tracker's
+# fused-pyramid ray cast (raycast_kernel<false, ...>) and of its shift boxes at such a side; its 21.9 cm threshold puts two shifts inside
+# the horizon.  There the raised millimetre of frame 1 changes no fused voxel, so ref' stays bit-identical to ref and measures nothing: the
+# horizon is bounded by the scene's, measured at 512^3 (frame 46, where only the back wall stays in view).
+@pytest.mark.parametrize("V,odometry,nframes,min_cmp,horizon_bound", [
+    pytest.param(512, 0, 72, 3, None, id="0-72"), pytest.param(512, 2, 22, 1, None, id="2-22"), pytest.param(512, 1, 26, 1, None, id="1-26"),
+    pytest.param(384, 0, 72, 2, 46, id="384-0-72")])
+def test_baseline_config_512_live_replay_exact(built, frames26, V, odometry, nframes, min_cmp, horizon_bound):
     import kintinuous_b200 as kb
     from conftest import GOLDEN
-    g = np.load(os.path.join(GOLDEN, f"ref_baseline_512_odo{odometry}.npz"))
+    g = np.load(os.path.join(GOLDEN, f"ref_baseline_{V}_odo{odometry}.npz"))
     cfg = kb.Config.default(vol=V, odometry=odometry)                  # voxel_shift 14, overlap 2: BASELINE configs[1] / configs[2]
     assert cfg.voxel_shift == 14 and cfg.overlap == 2
     mine = kb.Tracker(cfg)
@@ -96,7 +105,7 @@ def test_baseline_config_512_live_replay_exact(built, frames26, odometry, nframe
         if perturbed:
             gq, wp = g["poses_perturbed"][k][12:15], g["wraps_perturbed"][k]
             self_dev = float(np.abs(gq - gb).max())
-            if horizon is None and (self_dev > 2e-5 or not (wp == wb).all()):
+            if horizon is None and (self_dev > 2e-5 or not (wp == wb).all() or k == horizon_bound):
                 horizon = k; slices_at_horizon = n_slices
                 print(f"stable horizon K* = {k}: the reference moved {self_dev:.2e} m under a 1-LSB change of one depth pixel of frame 1")
             if horizon is None:
@@ -146,7 +155,7 @@ def test_baseline_config_512_live_replay_exact(built, frames26, odometry, nframe
             n_slices += 1
             shifted_frames.append(k)
         Rinv, tint, wint = mine.last_integrate()
-        assert list(wint) == (vwrap_nonneg(cur) if k > 0 else [0, 0, 0])
+        assert list(wint) == (vwrap_nonneg(cur, V) if k > 0 else [0, 0, 0])
         same_poses = same_poses and digest.raw(np.concatenate([Rinv.reshape(-1), tint, wint.astype(np.float32)])) == g["integrate_pose"][k]
     # the replay with the reference's operators used the integration poses recorded with the fixture; given the same poses, slices and
     # volume must be bit-identical to it (a change to the poses themselves is held to statement 1 and needs the fixture recorded again)
@@ -162,7 +171,7 @@ def test_baseline_config_512_live_replay_exact(built, frames26, odometry, nframe
     ta_, ca_ = mine.export_volume()
     if odometry == 0:
         assert n_slices >= 4, n_slices
-        assert n_cmp >= 3, n_cmp                                        # three shifts inside the stable horizon
+        assert n_cmp >= min_cmp, n_cmp                                  # shifts inside the stable horizon
         # 3b. the leaving slabs of this stream are mostly free space (the camera moves away from what it saw), so a slab that certainly
         # contains surface is extracted as well: 30 z planes around the room's back wall, on the product's volume at the final cyclic
         # offset, product operator against the reference's extractCloudSlice on the replayed volume -- the same multiset of points.
@@ -174,7 +183,7 @@ def test_baseline_config_512_live_replay_exact(built, frames26, odometry, nframe
         ts = torch.from_numpy(ta_.reshape(-1)).cuda(); cs = torch.from_numpy(ca_.reshape(-1)).cuda()
         oa = torch.zeros(cap * 32, dtype=torch.uint8, device="cuda")
         vs = [SIZE] * 3
-        n_a = kb.ops.extract_slice(ts, vs, V, oa, cap, vwrap_nonneg(cur), cs, box, 1, tuple(cur))
+        n_a = kb.ops.extract_slice(ts, vs, V, oa, cap, vwrap_nonneg(cur, V), cs, box, 1, tuple(cur))
         n_b = int(g["wall_n"])
         assert n_a == n_b and n_a > 20000, (n_a, n_b, box)
         from oracle import refbind
@@ -185,7 +194,7 @@ def test_baseline_config_512_live_replay_exact(built, frames26, odometry, nframe
         a, dim_a, _ = mine.get_slice(i); dim_b, len_b = (int(x) for x in g["ref_slices"][i])
         assert dim_a == dim_b and abs(len(a) - len_b) <= 0.01 * len_b + 5, (i, len(a), len_b)
     touched = int(g["replay_touched"])
-    assert touched > 1_000_000
+    assert touched > 1_000_000 * (V / 512) ** 3
     # 2. every voxel -- TSDF, weights and colours -- bit-identical to the replay of the product's poses through the reference's operators
     assert digest.raw(ta_.reshape(-1)) == g["replay_tsdf"], (odometry, "TSDF differs from the replay with the reference's operators")
     assert digest.raw(ca_.reshape(-1, 4)) == g["replay_color"], (odometry, "colour / weight differ from the replay with the reference's operators")

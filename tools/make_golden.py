@@ -4,7 +4,8 @@ by oracle/build_ref.sh from the reference sources) on an H100.  The reference sh
 so these fixtures are what pins the CPU oracle and the GPU parity tests: they are outputs of the reference itself on seeded
 synthetic input.
 
-Run on a GPU machine:   python tools/make_golden.py [OUT]        (writes OUT, default golden_out/, then copy to tests/golden/)
+Run on a GPU machine:   python tools/make_golden.py [OUT [PART ...]]   (writes OUT, default golden_out/, then copy to tests/golden/)
+PART records one group of fixtures only: `views` (ref_views_*.npz) or `baseline384` (ref_baseline_384_odo0.npz); default: all.
 Inputs are re-derivable from kintinuous_b200/synth.py (seed 20260922), so only outputs + a few parameters are stored; outputs
 too large to keep are stored as digests (tests/digest.py) or as a seeded sample.
 """
@@ -17,6 +18,7 @@ sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 sys.path.insert(0, os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "tests"))
 import torch  # noqa: E402
 import digest  # noqa: E402
+import volume_views  # noqa: E402
 import kintinuous_b200 as kb  # noqa: E402
 from kintinuous_b200 import synth  # noqa: E402
 from oracle import refbind  # noqa: E402
@@ -32,6 +34,11 @@ def dev(a):
 
 def main():
     os.makedirs(OUT, exist_ok=True)
+    parts = sys.argv[2:]
+    if parts:
+        for part in parts:
+            {"views": views, "baseline384": lambda: baseline(384, 0, 72)}[part]()
+        return
     ref = refbind.RefCuda(V)
     # ---------------- operator fixtures at 160 x 120 ----------------
     rows, cols = 120, 160
@@ -183,7 +190,9 @@ def live(ref):
     wrap_160(ref)
     tracker_live_256(ref)
     for odometry, nframes in ((0, 72), (2, 22), (1, 26)):
-        baseline_512(odometry, nframes)
+        baseline(512, odometry, nframes)
+    baseline(384, 0, 72)
+    views()
 
 
 def _front(ref, dd, rows, cols, intr):
@@ -366,17 +375,16 @@ def tracker_live_256(ref):
     np.savez_compressed(os.path.join(OUT, "ref_degenerate_256.npz"), **h)
 
 
-def baseline_512(odometry, nframes):
-    """test_baseline_config_512_live_replay_exact: BASELINE configs 1-2 (640x480 into 512^3, -t 14).  Records the reference tracker
+def baseline(vol, odometry, nframes):
+    """test_baseline_config_live_replay_exact: BASELINE configs 1-2 (640x480 into 512^3, -t 14), and ICP-only at 384^3 (not a power of two).  Records the reference tracker
     (and, ICP-only, its twin fed a 1-LSB perturbed frame 1), the reference operators' front end of every frame, and the replay of the
     PRODUCT's integration poses through the reference's operators: slices at every shift, the back-wall slab, the final volume."""
-    W512 = 512
     ROWS, COLS = 480, 640
-    ref = refbind.RefCuda(W512)
+    ref = refbind.RefCuda(vol)
     from concurrent.futures import ProcessPoolExecutor
     with ProcessPoolExecutor(max_workers=min(16, os.cpu_count() or 1)) as ex:
         frames = list(ex.map(synth.render, range(nframes), chunksize=2))
-    cfg = kb.Config.default(vol=W512, odometry=odometry)
+    cfg = kb.Config.default(vol=vol, odometry=odometry)
     mine = kb.Tracker(cfg)
     rt = ref.tracker(refbind.TrackerConfig.from_kt(cfg))
     rp = ref.tracker(refbind.TrackerConfig.from_kt(cfg)) if odometry == 0 else None
@@ -384,7 +392,7 @@ def baseline_512(odometry, nframes):
     vs = [SIZE] * 3
     g = {"trunc": np.float32(rt.trunc_dist)}
     trunc = mine.trunc_dist
-    ts = _z((W512 ** 3,), torch.int16); cs = _z((W512 ** 3 * 4,), torch.uint8)
+    ts = _z((vol ** 3,), torch.int16); cs = _z((vol ** 3 * 4,), torch.uint8)
     ref.init_volume(ts, cs)
     fb = _z((ROWS, COLS), torch.int16); vm = _z((3 * ROWS, COLS), torch.float32); nm = torch.zeros_like(vm); ds = _z((ROWS, COLS), torch.float32)
     cap = 3 * ROWS * COLS
@@ -411,15 +419,15 @@ def baseline_512(odometry, nframes):
             n = int(wa[axis]) - cur[axis]
             if n == 0:
                 continue
-            lo, hi = [0, 0, 0], [W512, W512, W512]
+            lo, hi = [0, 0, 0], [vol, vol, vol]
             if n > 0:
                 lo[axis], hi[axis] = 0, n + 1 + cfg.overlap
             elif axis < 2:
-                lo[axis], hi[axis] = W512 + (n - cfg.overlap), W512
+                lo[axis], hi[axis] = vol + (n - cfg.overlap), vol
             else:
-                lo[axis], hi[axis] = W512 + (n - cfg.overlap) - 1, W512 - 1
+                lo[axis], hi[axis] = vol + (n - cfg.overlap) - 1, vol - 1
             box = (lo[0], hi[0], lo[1], hi[1], lo[2], hi[2])
-            vw = [int(x) if x >= 0 else W512 - ((-int(x)) % W512) for x in cur]
+            vw = [int(x) if x >= 0 else vol - ((-int(x)) % vol) for x in cur]
             cnt = ref.extract(ts, vs, ob, cap, vw, cs, box, 1, cur)
             sl.append((k, axis, n, cnt, digest.raw(digest.canon(ob.cpu().numpy().view(refbind.POINT_DTYPE)[:cnt]))))
             ref.clear(axis, 1 if n < 0 else 0, ts, cs, cur[axis], cur[axis] + n)
@@ -433,9 +441,9 @@ def baseline_512(odometry, nframes):
     g["bilateral"] = np.array(FB); g["vmap"] = np.array(VM); g["nmap"] = np.array(NM); g["integrate_pose"] = np.array(INTEG)
     g["slice_events"] = np.array([s[:4] for s in sl], np.int64).reshape(-1, 4); g["slice_points"] = np.array([s[4] for s in sl])
     if odometry == 0:
-        wall = int((5.5 - cur[2] * SIZE / W512) / (SIZE / W512))
-        box = (0, W512, 0, W512, max(0, wall - 15), min(W512 - 1, wall + 15))
-        vw = [int(x) if x >= 0 else W512 - ((-int(x)) % W512) for x in cur]
+        wall = int((5.5 - cur[2] * SIZE / vol) / (SIZE / vol))
+        box = (0, vol, 0, vol, max(0, wall - 15), min(vol - 1, wall + 15))
+        vw = [int(x) if x >= 0 else vol - ((-int(x)) % vol) for x in cur]
         n_b = ref.extract(ts, vs, ob, cap, vw, cs, box, 1, cur)
         g["wall_box"] = np.array(box, np.int64); g["wall_n"] = np.int64(n_b)
         g["wall_points"] = np.array(digest.raw(digest.canon(ob.cpu().numpy().view(refbind.POINT_DTYPE)[:n_b])))
@@ -451,8 +459,71 @@ def baseline_512(odometry, nframes):
     mine.close(); rt.close()
     if rp is not None:
         rp.close()
-    np.savez_compressed(os.path.join(OUT, f"ref_baseline_512_odo{odometry}.npz"), **g)
-    print("baseline", odometry, "slices", len(sl), flush=True)
+    np.savez_compressed(os.path.join(OUT, f"ref_baseline_{vol}_odo{odometry}.npz"), **g)
+    print("baseline", vol, odometry, "slices", len(sl), flush=True)
+
+
+class _RefOps:
+    """The reference's operators with the product's argument order (the product's take the volume side, the reference's have it compiled in)."""
+
+    def __init__(self, ref):
+        self.r = ref
+        self.empty = None
+        self.racy = False
+
+    def init_volume(self, ts, cs, vol): self.r.init_volume(ts, cs)
+    def bilateral(self, src, dst, rows, cols): self.r.bilateral(src, dst, rows, cols)
+    def create_vmap(self, intr, depth, vmap, rows, cols): self.r.vmap(depth, vmap, rows, cols, intr)
+    def create_nmap(self, vmap, nmap, rows, cols): self.r.nmap(vmap, nmap, rows, cols)
+
+    def integrate(self, dd, rows, cols, intr, vs, Rinv, t, trunc, ts, cs, vol, wrap, rgb, nmap, angle_color, ds):
+        self.r.integrate(dd, rows, cols, intr, vs, Rinv, t, trunc, ts, cs, wrap, rgb, nmap, angle_color, ds)
+
+    def raycast(self, intr, R, t, trunc, vs, ts, vol, vmap, nmap, rows, cols, wrap, vmap_color, cs):
+        self.r.raycast(intr, R, t, trunc, vs, ts, vmap, nmap, rows, cols, wrap, vmap_color, cs)
+
+    def extract_slice(self, ts, vs, vol, out, cap, wrap, cs, box, subsample, real_wrap):
+        """The reference's extraction where it is well defined.  extract.cu:290-305 publishes the count from warp 0 of the last CTA and
+        resets it while other warps may still append (R1): their points land over the first ones, or are lost, or are counted into the
+        NEXT call.  A second call over a volume with no observed voxel (it appends nothing) publishes that remainder; a run is taken when
+        the remainder is 0, no point lies past the count (the buffer is zeroed first; a point's alpha, its weight, is never 0) and a second
+        such run gives the same count and points (at most 16 tries).  Otherwise self.racy is set and the
+        slab is not recorded."""
+        import torch
+        if self.empty is None or self.empty[0].numel() != vol ** 3:
+            self.empty = (torch.zeros(vol ** 3, dtype=torch.int16, device="cuda"), torch.zeros(vol ** 3 * 4, dtype=torch.uint8, device="cuda"))
+        spare = torch.zeros(32 * 16, dtype=torch.uint8, device="cuda")
+        seen = set()
+        self.racy = True
+        for _ in range(16):
+            out.zero_()
+            n = self.r.extract(ts, vs, out, cap, wrap, cs, box, subsample, real_wrap)
+            # (capacity `cap`: the count is clamped to it; the empty volume writes no point into the small buffer)
+            late = self.r.extract(self.empty[0], vs, spare, cap, (0, 0, 0), self.empty[1], (0, vol, 0, vol, 0, 8), 1, (0, 0, 0))
+            # a point appended after the count was published but before the reset is written past it, uncounted
+            if late or (n < cap and int(out[n * 32 + 19].item()) != 0):
+                continue
+            key = (n, digest.raw(digest.canon(out[:n * 32].cpu().numpy().reshape(n, 32))) if n else "")
+            if key in seen:
+                self.racy = False
+                return n
+            seen.add(key)
+        return n
+
+    def clear_volume(self, axis, back, ts, cs, vol, current, delta): self.r.clear(axis, back, ts, cs, current, delta)
+
+
+def views():
+    """test_gpu_volume_views.py: the reference's operators over tests/volume_views.py's table of views, one file per (V, volume size).
+    Every extraction box is a slab, never the whole volume (R1: a whole-volume extraction can leak counts into the next call)."""
+    for vol, vs, names in volume_views.table():
+        ref = refbind.RefCuda(vol)
+        g = volume_views.run_case(_RefOps(ref), torch, vol, vs, names)
+        for n in names:
+            print(vol, vs, n, "touched", g[f"{n}.touched"], "hits", g[f"{n}.ray0_hits"], g[f"{n}.ray1_hits"],
+                  "extract", [g.get(f"{n}.ext_{b}_n", "racy") for b in volume_views.slabs(vol)], flush=True)
+        np.savez_compressed(os.path.join(OUT, f"ref_views_{volume_views.case_key(vol, vs)}.npz"), **g)
+        torch.cuda.empty_cache()
 
 
 if __name__ == "__main__":
