@@ -263,6 +263,42 @@ typedef struct kt_weld_report {
 KT_API int kt_get_map_mesh(kt_ctx* ctx, int which, int weld, kt_mesh_vertex* verts, size_t max_verts, uint32_t* tris, size_t max_tris,
                            size_t* n_verts, size_t* n_tris, kt_weld_report* report);
 KT_API int kt_save_map_ply(kt_ctx* ctx, const char* path, int which, int weld, kt_weld_report* report);
+/* The map volume (no counterpart in the reference, which meshes point slices with PCL's GP3): a sparse global TSDF kept on the device,
+ * so that the whole map is meshed in ONE marching-cubes pass over one consistent field and no seam is left open where the surface moved
+ * between two slices (the weld above cannot close those: the values that would decide them were cleared at the shift).
+ *   - Just before each shift clears its storage planes, the surface voxels of those planes (W != 0 and F != 1) get their 8^3 brick, and
+ *     every cleared voxel with W != 0 overwrites its value in a brick that exists: each global voxel keeps its latest observation, and
+ *     free space observed later removes an old surface.  A global voxel is the logical voxel plus the real voxel wrap (the index of
+ *     kt_get_slice_mesh_keys).  Bricks are keyed (bz + 2^20) << 42 | (by + 2^20) << 21 | (bx + 2^20) (21 signed bits per axis, z most
+ *     significant); voxel (x, y, z) of brick b is global voxel 8 b + (x, y, z), stored at x + 8 y + 64 z.
+ *   - Capacity is all or nothing per cleared slab: when a slab's new bricks do not all fit, none is stored (bricks already stored are
+ *     still updated), `full` is set and tracking carries on.  Three kernel launches per cleared slab on the tracker stream, no host synchronisation; frames without a shift launch
+ *     nothing more.  Off by default.
+ * kt_set_map_volume(ctx, 1, max_bricks) allocates an empty store of max_bricks bricks (3 KB each plus 24 B of hash per brick) up front,
+ * replacing any current one; KT_ERR_CUDA when the memory is refused, and then nothing else changes.  enabled = 0 frees it.  kt_reset
+ * empties it.  KT_ERR_INVALID for a volume shared by several GPUs (world > 1); the calls below return KT_ERR_STATE while it is off. */
+KT_API int kt_set_map_volume(kt_ctx* ctx, int enabled, size_t max_bricks);
+KT_API int kt_get_map_volume_info(kt_ctx* ctx, size_t* bricks, size_t* capacity, int* full);
+/* The stored bricks sorted by key: keys, tsdf (512 int16 per brick) and colour (512 x 4 uint8: b, g, r, weight per voxel, the volume's
+ * layout); any output may be NULL.  *n_bricks = the count; KT_ERR_CAPACITY (nothing copied) when it exceeds max_bricks. */
+KT_API int kt_get_map_volume_bricks(kt_ctx* ctx, uint64_t* keys, int16_t* tsdf, uint8_t* color, size_t max_bricks, size_t* n_bricks);
+/* The whole map's mesh: kt_op_mesh_bricks over S, the store where the live volume has W = 0 and the live volume elsewhere (the live
+ * volume is read, nothing is modified, so an export mid-run changes nothing that follows).  Corners need alpha >= weight_cull.  Vertices
+ * ascend by (owning global voxel in (z, y, x) order, edge axis), triangles by cell in that order, then in table order: a run that never
+ * shifted gives kt_get_live_mesh's bytes.  The store is in tracked coordinates (there is no corrected variant).  Copies up to max_verts /
+ * max_tris (NULL outputs: counts only) and returns both counts; synchronous, on the tracker stream, scratch freed before returning.
+ * kt_save_global_mesh_ply writes the same mesh in kt_save_mesh_ply's binary PLY layout. */
+typedef struct kt_global_mesh_report {
+    size_t bricks;                      /* bricks meshed: the store's and the live volume's surface bricks, each once */
+    size_t store_bricks, live_bricks;
+    size_t input_voxels;                /* bricks x 512 */
+    size_t output_verts, output_tris;
+    int store_full;                     /* a shift's bricks did not fit the store (kt_get_map_volume_info's full) */
+    float gather_ms, mesh_ms, sort_ms, download_ms, total_ms;   /* CUDA-event times: merge of store and live volume; count + emit; sorts */
+} kt_global_mesh_report;
+KT_API int kt_get_global_mesh(kt_ctx* ctx, int weight_cull, kt_mesh_vertex* verts, size_t max_verts, uint32_t* tris, size_t max_tris,
+                              size_t* n_verts, size_t* n_tris, kt_global_mesh_report* report);
+KT_API int kt_save_global_mesh_ply(kt_ctx* ctx, const char* path, int weight_cull, kt_global_mesh_report* report);
 /* Loop closure: the pose-graph half of the reference's backend (backend/Deformation.cpp:130-346 addCameraCamera / addCameraLoop,
  * backend/iSAMInterface.cpp) on the GPU.  The caller passes what PlaceRecognition produces (LoopClosureConstraint,
  * PlaceRecognition.cpp:198-209): time1 (the new frame) and time2 (the old one), both dense pose timestamps, the pose of the camera at
@@ -502,6 +538,14 @@ KT_API int kt_op_mesh_volume_keyed(const int16_t* tsdf_dev, const uint8_t* color
                                    const int* voxel_wrap3, const int* real_voxel_wrap3, int minX, int maxX, int minY, int maxY, int minZ, int maxZ,
                                    int weight_cull, kt_mesh_vertex* verts_dev, int32_t* vert_edges_dev, size_t max_verts, uint32_t* tris_dev,
                                    int32_t* tri_cells_dev, size_t max_tris, size_t* n_verts, size_t* n_tris, void* stream);
+/* Marching cubes over a sparse set of 8^3 bricks (device): keys strictly ascending (kt_set_map_volume's key layout), 512 int16 tsdf and
+ * 512 x 4 uint8 colour per brick.  kt_op_mesh_volume's contract with the global voxel as the logical one and no border: a voxel outside
+ * every brick is unobserved.  Positions as kt_op_mesh_volume's with real_voxel_wrap 0 and this vol (cell = volume_size3 / vol); the
+ * order is kt_get_global_mesh's.  NULL outputs: counts only; KT_ERR_CAPACITY (nothing written) when they exceed the capacities;
+ * KT_ERR_INVALID for unsorted keys.  Synchronous. */
+KT_API int kt_op_mesh_bricks(const uint64_t* keys_dev, const int16_t* tsdf_dev, const uint8_t* color_dev, size_t n_bricks, const float* volume_size3,
+                             int vol, int weight_cull, kt_mesh_vertex* verts_dev, size_t max_verts, uint32_t* tris_dev, size_t max_tris,
+                             size_t* n_verts, size_t* n_tris, void* stream);
 /* Weld n_meshes keyed meshes (kt_op_mesh_volume_keyed, kt_get_slice_mesh_keys) into one (kt_weld.cu).  Input (device): the meshes
  * concatenated in order -- vertices with their edges, triangles (indices local to their own mesh) with their cells -- and n_meshes + 1
  * HOST offsets of each mesh's first vertex / triangle (vert_offsets_host[n_meshes] = all vertices).

@@ -167,6 +167,16 @@ class WeldReport(C.Structure):
         return {k: getattr(self, k) for k, _ in self._fields_}
 
 
+class GlobalMeshReport(C.Structure):
+    """kt_global_mesh_report of kt_get_global_mesh / kt_save_global_mesh_ply."""
+    _fields_ = [("bricks", C.c_size_t), ("store_bricks", C.c_size_t), ("live_bricks", C.c_size_t), ("input_voxels", C.c_size_t),
+                ("output_verts", C.c_size_t), ("output_tris", C.c_size_t), ("store_full", C.c_int), ("gather_ms", C.c_float),
+                ("mesh_ms", C.c_float), ("sort_ms", C.c_float), ("download_ms", C.c_float), ("total_ms", C.c_float)]
+
+    def as_dict(self):
+        return {k: getattr(self, k) for k, _ in self._fields_}
+
+
 class SliceInfo(C.Structure):
     _fields_ = [("dimension", C.c_int), ("odometry", C.c_int), ("camera_t", C.c_float * 3), ("camera_R", C.c_float * 9),
                 ("utime", C.c_uint64), ("count", C.c_size_t)]
@@ -337,6 +347,43 @@ class Tracker:
         """The same mesh as a binary PLY in save_mesh_ply's layout (kt_save_map_ply).  Returns the report dict."""
         rep = WeldReport()
         _check(self.lib.kt_save_map_ply(self.h, os.fsencode(path), int(which), int(weld), C.byref(rep)))
+        return rep.as_dict()
+
+    def set_map_volume(self, enabled=True, max_bricks=1 << 16):
+        """The map volume (kt_set_map_volume): a sparse global TSDF of every voxel a shift clears, in 8^3 bricks; 0 frees it."""
+        _check(self.lib.kt_set_map_volume(self.h, int(enabled), C.c_size_t(max_bricks)))
+
+    def map_volume_info(self):
+        """(bricks stored, capacity, full) of the map volume."""
+        b = C.c_size_t(0); cap = C.c_size_t(0); full = C.c_int(0)
+        _check(self.lib.kt_get_map_volume_info(self.h, C.byref(b), C.byref(cap), C.byref(full)))
+        return b.value, cap.value, bool(full.value)
+
+    def map_volume_bricks(self):
+        """The stored bricks sorted by key: (keys uint64 [n], tsdf int16 [n, 8, 8, 8], colour uint8 [n, 8, 8, 8, 4]), voxels indexed [z, y, x]."""
+        n = C.c_size_t(0)
+        _check(self.lib.kt_get_map_volume_bricks(self.h, None, None, None, C.c_size_t(0), C.byref(n)))
+        k = np.zeros(n.value, np.uint64); t = np.zeros((n.value, 8, 8, 8), np.int16); c = np.zeros((n.value, 8, 8, 8, 4), np.uint8)
+        if n.value:
+            _check(self.lib.kt_get_map_volume_bricks(self.h, _ptr(k), _ptr(t), _ptr(c), C.c_size_t(len(k)), C.byref(n)))
+        return k, t, c
+
+    def global_mesh(self, weight_cull=8):
+        """The whole map as one mesh from the map volume and the live volume (kt_get_global_mesh): (vertices, triangles [m, 3], report
+        dict).  Counts first, then fetches: that runs the export twice."""
+        nv = C.c_size_t(0); nt = C.c_size_t(0); rep = GlobalMeshReport()
+        _check(self.lib.kt_get_global_mesh(self.h, int(weight_cull), None, C.c_size_t(0), None, C.c_size_t(0), C.byref(nv), C.byref(nt), C.byref(rep)))
+        v = np.zeros(nv.value, MESH_VERTEX_DTYPE); t = np.zeros((nt.value, 3), np.uint32)
+        if nv.value or nt.value:
+            _check(self.lib.kt_get_global_mesh(self.h, int(weight_cull), _ptr(v), C.c_size_t(len(v)), _ptr(t), C.c_size_t(len(t)),
+                                               C.byref(nv), C.byref(nt), C.byref(rep)))
+        assert (nv.value, nt.value) == (len(v), len(t))
+        return v, t, rep.as_dict()
+
+    def save_global_mesh_ply(self, path, weight_cull=8):
+        """The same mesh as a binary PLY in save_mesh_ply's layout (kt_save_global_mesh_ply).  Returns the report dict."""
+        rep = GlobalMeshReport()
+        _check(self.lib.kt_save_global_mesh_ply(self.h, os.fsencode(path), int(weight_cull), C.byref(rep)))
         return rep.as_dict()
 
     def live_mesh(self):
@@ -712,6 +759,30 @@ class _Ops:
         assert (nv2, nt2) == (nv, nt)
         return (v.cpu().numpy().view(MESH_VERTEX_DTYPE).copy(), t[:3 * nt].cpu().numpy().view(np.uint32).reshape(nt, 3).copy(),
                 e.cpu().numpy().reshape(nv, 4), k[:4 * nt].cpu().numpy().reshape(nt, 4))
+
+    def mesh_bricks_into(self, keys_dev, tsdf_dev, color_dev, n_bricks, volume_size, vol, weight_cull, verts_dev, max_verts, tris_dev, max_tris):
+        """kt_op_mesh_bricks into caller buffers: (status, n_verts, n_tris); status is 0 or KT_ERR_CAPACITY (nothing written)."""
+        vs = _f(volume_size)
+        nv = C.c_size_t(0); nt = C.c_size_t(0)
+        st = self._l().kt_op_mesh_bricks(_ptr(keys_dev), _ptr(tsdf_dev), _ptr(color_dev), C.c_size_t(n_bricks), _ptr(vs), int(vol), int(weight_cull),
+                                         _ptr(verts_dev), C.c_size_t(max_verts), _ptr(tris_dev), C.c_size_t(max_tris), C.byref(nv), C.byref(nt), None)
+        if st not in (0, KT_ERR_CAPACITY):
+            _check(st)
+        return st, nv.value, nt.value
+
+    def mesh_bricks(self, keys, tsdf, color, volume_size, vol, weight_cull=8):
+        """Marching cubes over a sorted brick set (kt_op_mesh_bricks): keys uint64 [n], tsdf int16 [n, 8, 8, 8], colour uint8 [n, 8, 8, 8, 4]
+        (host arrays or CUDA tensors).  Returns host arrays (vertices MESH_VERTEX_DTYPE [n], triangles uint32 [m, 3])."""
+        import torch
+        dev = lambda a: a if isinstance(a, torch.Tensor) else torch.from_numpy(np.ascontiguousarray(a).view(np.uint8).reshape(-1).copy()).cuda()  # noqa: E731
+        n = len(keys)
+        dk, dt, dc = (dev(keys), dev(tsdf), dev(color)) if n else (None, None, None)
+        _, nv, nt = self.mesh_bricks_into(dk, dt, dc, n, volume_size, vol, weight_cull, None, 0, None, 0)
+        v = torch.empty(max(nv, 1) * 32, dtype=torch.uint8, device="cuda"); t = torch.empty(max(nt, 1) * 3, dtype=torch.int32, device="cuda")
+        st, nv2, nt2 = self.mesh_bricks_into(dk, dt, dc, n, volume_size, vol, weight_cull, v, nv, t, nt)
+        _check(st)
+        assert (nv2, nt2) == (nv, nt)
+        return v[:32 * nv].cpu().numpy().view(MESH_VERTEX_DTYPE).copy(), t[:3 * nt].cpu().numpy().view(np.uint32).reshape(nt, 3).copy()
 
     def weld_meshes_into(self, verts_dev, edges_dev, vert_offsets, tris_dev, cells_dev, tri_offsets, out_verts_dev, max_verts, out_tris_dev, max_tris):
         """kt_op_weld_meshes on device buffers with host offsets (n_meshes + 1 each): (status, n_verts, n_tris, report dict); status is 0

@@ -249,6 +249,23 @@ int kt_op_mesh_volume_keyed(const int16_t* tsdf, const uint8_t* color, int vol, 
     return KT_OK;
 }
 
+int kt_op_mesh_bricks(const uint64_t* keys, const int16_t* tsdf, const uint8_t* color, size_t n_bricks, const float* vs, int vol, int weight_cull,
+                      kt_mesh_vertex* verts, size_t max_verts, uint32_t* tris, size_t max_tris, size_t* n_verts, size_t* n_tris, void* s)
+{
+    const char* who = "kt_op_mesh_bricks";
+    if (!vs || !n_verts || !n_tris || (n_bricks && (!keys || !tsdf || !color))) { set_error("%s: bad argument", who); return KT_ERR_INVALID; }
+    if (vol <= 0) { set_error("%s: vol %d is not positive", who, vol); return KT_ERR_INVALID; }
+    const MeshOutput out = [&](size_t nv, size_t nt, void** v, uint32_t** t) -> int {
+        if (!verts && !tris) return 1;
+        if (nv > max_verts || nt > max_tris || !verts || (nt && !tris)) {
+            set_error("%s: %zu vertices / %zu triangles exceed the capacities", who, nv, nt); return KT_ERR_CAPACITY; }
+        *v = verts; *t = tris;
+        return 0;
+    };
+    BrickSet set = {(const unsigned long long*)keys, tsdf, color, n_bricks};
+    return mesh_bricks(set, make_float3(vs[0], vs[1], vs[2]), vol, weight_cull, out, n_verts, n_tris, nullptr, st(s));
+}
+
 int kt_op_weld_meshes(const kt_mesh_vertex* verts, const int32_t* vert_edges, const size_t* vert_offsets, const uint32_t* tris, const int32_t* tri_cells,
                       const size_t* tri_offsets, int n_meshes, kt_mesh_vertex* out_verts, size_t max_verts, uint32_t* out_tris, size_t max_tris,
                       size_t* n_verts, size_t* n_tris, kt_weld_report* report, void* s)

@@ -36,7 +36,6 @@ namespace {
 const int MESH_THREADS = 256;
 const int MESH_ITEMS = 16;
 const long long MESH_TILE = (long long)MESH_THREADS * MESH_ITEMS;
-const unsigned int CELL_CORNERS = 0x361Bu;     // bits of the 8 corners of a cell in a 3x3x3 neighbourhood (index dx + 3 dy + 9 dz), cell at 0
 
 struct MeshParams {
     const int16_t* tsdf; const uchar4* color; int V; int3 wrap; int3 real_wrap; float3 cell, inv_cell; int cull;
@@ -69,48 +68,25 @@ __device__ __forceinline__ void owner_xyz(const MeshParams& p, long long idx, in
     z = p.minZ + (int)(r / p.ey);
 }
 
-// What the owner voxel idx contributes: the crossing edges it owns that a meshed cell uses (bit a = axis a) and, when cell (x, y, z)
-// is meshed, its case (else -1).
+// What the owner voxel idx contributes (mc_classify, kt_surface.cuh): cells are meshed inside the box and away from the far border
 struct Voxel { int x, y, z; unsigned int vflags; int mc_case; };
+
+// the volume as kt_surface.cuh's Field: logical voxels, no cyclic wrap
+struct BoxField {
+    const MeshParams& p;
+    __device__ __forceinline__ bool corner(int x, int y, int z, short& raw) const { return kt::corner(p, x, y, z, raw); }
+    __device__ __forceinline__ short raw(int x, int y, int z) const { return __ldg(&p.tsdf[vaddr(p, x, y, z)]); }
+    __device__ __forceinline__ uchar4 color(int x, int y, int z) const { return __ldg(&p.color[vaddr(p, x, y, z)]); }
+};
 
 __device__ __forceinline__ Voxel classify(const MeshParams& p, long long idx)
 {
-    Voxel v; owner_xyz(p, idx, v.x, v.y, v.z); v.vflags = 0; v.mc_case = -1;
-    short r;
-    if (!corner(p, v.x, v.y, v.z, r)) return v;           // an invalid voxel is no cell's corner and owns no edge
-    unsigned int valid = 0, inside = 0;
-#pragma unroll
-    for (int dz = -1; dz <= 1; ++dz)
-#pragma unroll
-        for (int dy = -1; dy <= 1; ++dy)
-#pragma unroll
-            for (int dx = -1; dx <= 1; ++dx) {
-                const int b = (dx + 1) + 3 * (dy + 1) + 9 * (dz + 1);
-                short q;
-                if (corner(p, v.x + dx, v.y + dy, v.z + dz, q)) { valid |= 1u << b; if (q < 0) inside |= 1u << b; }
-            }
-    // cell whose lower corner is (x + ox, y + oy, z + oz), o in {-1, 0}^3: in the box, inside [0, V - 1), 8 valid corners
-    auto cell_ok = [&](int ox, int oy, int oz) -> bool {
-        const int cx = v.x + ox, cy = v.y + oy, cz = v.z + oz;
-        if (cx < p.minX || cx >= p.maxX || cy < p.minY || cy >= p.maxY || cz < p.minZ || cz >= p.maxZ) return false;
-        if (cx + 1 >= p.V || cy + 1 >= p.V || cz + 1 >= p.V) return false;
-        const unsigned int m = CELL_CORNERS << ((ox + 1) + 3 * (oy + 1) + 9 * (oz + 1));
-        return (valid & m) == m;
-    };
-    if (cell_ok(0, 0, 0)) {
-        int c = 0;
-#pragma unroll
-        for (int k = 0; k < 8; ++k) c |= (int)((inside >> (13 + (k & 1) + 3 * ((k >> 1) & 1) + 9 * (k >> 2))) & 1u) << k;
-        if (c != 0 && c != 255) v.mc_case = c;
-    }
-    const bool in0 = (inside >> 13) & 1u;
-    // x edge: (x, y, z) - (x + 1, y, z), used by the cells at (x, y - dy, z - dz)
-    if (((valid >> 14) & 1u) && (((inside >> 14) & 1u) != in0) &&
-        (cell_ok(0, 0, 0) || cell_ok(0, -1, 0) || cell_ok(0, 0, -1) || cell_ok(0, -1, -1))) v.vflags |= 1u;
-    if (((valid >> 16) & 1u) && (((inside >> 16) & 1u) != in0) &&
-        (cell_ok(0, 0, 0) || cell_ok(-1, 0, 0) || cell_ok(0, 0, -1) || cell_ok(-1, 0, -1))) v.vflags |= 2u;
-    if (((valid >> 22) & 1u) && (((inside >> 22) & 1u) != in0) &&
-        (cell_ok(0, 0, 0) || cell_ok(-1, 0, 0) || cell_ok(0, -1, 0) || cell_ok(-1, -1, 0))) v.vflags |= 4u;
+    Voxel v; owner_xyz(p, idx, v.x, v.y, v.z);
+    const McVoxel m = mc_classify(BoxField{p}, v.x, v.y, v.z, [&](int cx, int cy, int cz) {
+        return cx >= p.minX && cx < p.maxX && cy >= p.minY && cy < p.maxY && cz >= p.minZ && cz < p.maxZ &&
+               cx + 1 < p.V && cy + 1 < p.V && cz + 1 < p.V;
+    });
+    v.vflags = m.vflags; v.mc_case = m.mc_case;
     return v;
 }
 
@@ -137,47 +113,9 @@ mesh_count_kernel(const MeshParams p, unsigned long long* vcount, unsigned long 
     }
 }
 
-// TSDF gradient at a valid voxel (raw r0), per metre, in raw units
-__device__ __forceinline__ float3 gradient(const MeshParams& p, int x, int y, int z, short r0)
-{
-    float g[3];
-    const float inv[3] = {p.inv_cell.x, p.inv_cell.y, p.inv_cell.z};
-#pragma unroll
-    for (int b = 0; b < 3; ++b) {
-        const int dx = b == 0, dy = b == 1, dz = b == 2;
-        short rm = 0, rp = 0;
-        const bool okm = corner(p, x - dx, y - dy, z - dz, rm), okp = corner(p, x + dx, y + dy, z + dz, rp);
-        g[b] = okm && okp ? (float)(rp - rm) * 0.5f * inv[b] : okp ? (float)(rp - r0) * inv[b] : okm ? (float)(r0 - rm) * inv[b] : 0.f;
-    }
-    return make_float3(g[0], g[1], g[2]);
-}
-
 __device__ __forceinline__ void write_vertex(const MeshParams& p, int x, int y, int z, int a, uint4* out)
 {
-    const int dx = a == 0, dy = a == 1, dz = a == 2;
-    const size_t a0 = vaddr(p, x, y, z), a1 = vaddr(p, x + dx, y + dy, z + dz);
-    const short r0 = __ldg(&p.tsdf[a0]), r1 = __ldg(&p.tsdf[a1]);
-    const float F = unpack_tsdf(r0), Fn = unpack_tsdf(r1);
-    // extract_kernel's point for this edge (kt_extract.cu), expression for expression
-    float3 Vc;
-    Vc.x = (x + 0.5f) * p.cell.x; Vc.y = (y + 0.5f) * p.cell.y; Vc.z = (z + 0.5f) * p.cell.z;
-    const float d_inv = 1.f / (fabs(F) + fabs(Fn));
-    if (a == 0) { float Vnx = Vc.x + p.cell.x; Vc.x = interp(Vc.x, Vnx, F, Fn, d_inv); }
-    else if (a == 1) { float Vny = Vc.y + p.cell.y; Vc.y = interp(Vc.y, Vny, F, Fn, d_inv); }
-    else { float Vnz = Vc.z + p.cell.z; Vc.z = interp(Vc.z, Vnz, F, Fn, d_inv); }
-    const float px = slice_coord(Vc.x, p.real_wrap.x, p.cell.x, p.V);
-    const float py = slice_coord(Vc.y, p.real_wrap.y, p.cell.y, p.V);
-    const float pz = slice_coord(Vc.z, p.real_wrap.z, p.cell.z, p.V);
-    const float3 g0 = gradient(p, x, y, z, r0), g1 = gradient(p, x + dx, y + dy, z + dz, r1);
-    const float w0 = fabsf(Fn) * d_inv, w1 = fabsf(F) * d_inv;
-    float3 n = make_float3(w0 * g0.x + w1 * g1.x, w0 * g0.y + w1 * g1.y, w0 * g0.z + w1 * g1.z);
-    const float l2 = n.x * n.x + n.y * n.y + n.z * n.z;
-    if (l2 > 0.f) { const float s = rsqrtf(l2); n.x *= s; n.y *= s; n.z *= s; } else n = make_float3(0.f, 0.f, 0.f);
-    const bool lower = abs((int)r0) <= abs((int)r1);
-    const uchar4 c = __ldg(&p.color[lower ? a0 : a1]);
-    const unsigned int rgba = (unsigned int)c.z | ((unsigned int)c.y << 8) | ((unsigned int)c.x << 16) | ((unsigned int)c.w << 24);
-    out[0] = make_uint4(__float_as_uint(px), __float_as_uint(py), __float_as_uint(pz), __float_as_uint(n.x));
-    out[1] = make_uint4(__float_as_uint(n.y), __float_as_uint(n.z), rgba, 0u);
+    mc_vertex(BoxField{p}, p.cell, p.inv_cell, p.real_wrap, p.V, x, y, z, a, out);
 }
 
 __global__ void __launch_bounds__(MESH_THREADS)

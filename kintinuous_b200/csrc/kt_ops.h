@@ -3,10 +3,12 @@
 #pragma once
 #include "kt_common.cuh"
 #include "kt_mem.hpp"
+#include <functional>
 
 struct kt_deform_report;
 struct kt_pgo_report;
 struct kt_weld_report;
+struct kt_global_mesh_report;
 
 namespace kt {
 
@@ -140,6 +142,8 @@ int init_shared(const VolumeView& vv, int vol, cudaStream_t s);       // this ra
 int clear_volume(int axis, int back, int16_t* tsdf, uint8_t* color, int vol, int current_wrap, int delta_wrap, cudaStream_t s);
 // shared volume: the TSDF planes of the local replica and the colour planes this rank owns
 int clear_volume_shared(int axis, int back, const VolumeView& vv, int vol, int current_wrap, int delta_wrap, cudaStream_t s);
+// the storage planes [first, first + planes) (mod vol) along `axis` that clear_volume zeroes (SURVEY.md Q13: an x clear reaches round_up_16)
+void clear_range(int axis, int back, int vol, int current_wrap, int delta_wrap, int* first, int* planes);
 int scale_depth(const uint16_t* depth, float* scaled, int rows, int cols, const Intr& k, bool angle_color, cudaStream_t s);
 struct IntegrateArgs {
     const float* depth_scaled; int rows, cols; Intr k; float3 volume_size; Mat33 Rinv; float3 t; float trunc;
@@ -267,6 +271,38 @@ int rigid_move_mesh(void* verts_dev, size_t n, const RigidF& C, cudaStream_t s);
 int weld_meshes(const void* verts, const int32_t* vert_edges, const size_t* voff, const uint32_t* tris, const int32_t* tri_cells, const size_t* toff,
                 int n_meshes, void* out_verts, size_t max_verts, uint32_t* out_tris, size_t max_tris, size_t* n_verts, size_t* n_tris,
                 kt_weld_report* rep, cudaStream_t s);
+// ---- map volume (kt_mapvol.cu): a sparse global TSDF of the voxels the shifts clear, 8^3 bricks behind a hash; see the file header ----
+static const int MAPVOL_BRICK_VOXELS = 512;      // voxel (x, y, z) of a brick at x + 8 y + 64 z
+static const int MAPVOL_COORD_BIAS = 1 << 20;    // brick key: (bz + bias) << 42 | (by + bias) << 21 | (bx + bias), 21 bits per axis
+struct MapVolume {
+    Allocations mem;
+    unsigned int capacity = 0, slots = 0;                                    // bricks; hash slots (a power of two >= 2 capacity)
+    unsigned long long* slot_key = nullptr; unsigned int* slot_val = nullptr;  // open addressing, empty = ~0; value = pool index
+    unsigned long long* brick_key = nullptr;                                 // pool index -> key
+    int16_t* tsdf = nullptr; uint8_t* color = nullptr;                       // pool: 512 voxels per brick
+    unsigned int* state = nullptr; unsigned int* state_host = nullptr;       // bricks taken, committed, refused, full
+};
+// allocates everything up front (KT_ERR_CUDA when refused) and empties it
+int mapvol_init(MapVolume* m, size_t max_bricks, cudaStream_t s);
+int mapvol_empty(MapVolume* m, cudaStream_t s);
+// before a clear of storage planes [first, first + planes) along axis (clear_range): keep their voxels; wrap = the signed voxel wrap.
+// Three launches, asynchronous.
+int mapvol_store(MapVolume* m, const int16_t* tsdf, const uint8_t* color, int vol, const int* wrap, int axis, int first, int planes, cudaStream_t s);
+int mapvol_info(MapVolume* m, size_t* bricks, int* full, cudaStream_t s);          // synchronises s
+// the store sorted by key into host arrays (any may be null); *n = bricks; KT_ERR_CAPACITY beyond max.  Synchronises s.
+int mapvol_bricks(MapVolume* m, unsigned long long* keys, int16_t* tsdf, uint8_t* color, size_t max, size_t* n, cudaStream_t s);
+// Where a mesh goes once its counts are known: return 0 with device pointers for nv vertices and nt triangles, 1 for the counts alone,
+// or a negative kt_status.
+using MeshOutput = std::function<int(size_t nv, size_t nt, void** verts, uint32_t** tris)>;
+struct BrickSet { const unsigned long long* keys; const int16_t* tsdf; const uint8_t* color; size_t n; };   // device, keys strictly ascending
+// marching cubes over a brick set (kt_mesh.cu's contract with the global voxel as the logical one, no border; positions with real wrap
+// 0 and centred by vol); ms (may be null): device ms of count + emit, of the sorts, in all.  Scratch per call; synchronises s.
+int mesh_bricks(const BrickSet& set, const float3& volume_size, int vol, int weight_cull, const MeshOutput& out, size_t* n_verts, size_t* n_tris,
+                float* ms, cudaStream_t s);
+// the map mesh: mesh_bricks over the store merged with the live volume (wrap = the signed voxel wrap); every field of the report but
+// download_ms.  Synchronises s.
+int mapvol_mesh(const MapVolume* m, const int16_t* tsdf, const uint8_t* color, int vol, const int* wrap, const float3& volume_size, int weight_cull,
+                const MeshOutput& out, size_t* n_verts, size_t* n_tris, kt_global_mesh_report* rep, cudaStream_t s);
 // cross-GPU barrier: every rank writes `epoch` into slot [rank] of every peer's flag array, then waits until all slots of its own
 // array reach `epoch` (bounded spin: returns through *error_dev != 0 instead of hanging the GPU if a peer never arrives)
 int xgpu_barrier(unsigned int* const* peer_flags_dev /* [world] device array of pointers */, unsigned int* my_flags, int rank, int world,

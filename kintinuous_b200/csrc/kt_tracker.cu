@@ -243,6 +243,7 @@ struct kt_ctx {
     float last_int_Rinv[9], last_int_t[3]; int last_int_wrap[3];       // arguments of the last integration (kt_debug_last_integrate)
     DeviceBuffer<uint8_t> view;                                         // GUI taps: shaded image, colour image, model depth (allocated on first use)
     std::unique_ptr<PlaceStore> place;                                  // loop detection (null while it is off)
+    std::unique_ptr<MapVolume> mapvol;                                  // the map volume (kt_mapvol.cu; null while it is off)
     // what member destructors cannot do: wait for the streams, unmap the peers' arenas, close the pose log
     ~kt_ctx()
     {
@@ -646,6 +647,11 @@ int process_frame_device(kt_ctx* c, uint64_t utime, kt_pose* out)
             if ((r = fetch_cloud(c, vWrapCopy, lo, hi))) return r;
             if (c->slice_meshing && (r = mesh_box(c, vWrapCopy, lo, hi, true))) return r;
             if ((r = mg_barrier(c))) return r;                          // peers may still read my boundary plane for their extraction
+            if (c->mapvol) {                                            // keep what the clear is about to zero
+                int first, planes;
+                clear_range(axis, dir < 0 ? 1 : 0, V, c->voxelWrap[axis], c->voxelWrap[axis] + n, &first, &planes);
+                if ((r = mapvol_store(c->mapvol.get(), c->tsdf, c->color, V, c->voxelWrap, axis, first, planes, c->stream))) return r;
+            }
             if ((r = clear_volume_shared(axis, dir < 0 ? 1 : 0, c->vv, V, c->voxelWrap[axis], c->voxelWrap[axis] + n, c->stream))) return r;
         }
         if (cycled) {                                                                    // mutexOutCloudBuffer (.cpp:1156-1208)
@@ -724,6 +730,7 @@ int kt_cuda_available(void)
 int kt_reset(kt_ctx* c)
 {
     if (!c) return KT_ERR_INVALID;
+    int r0;
     c->global_time = 0;
     c->rmats.clear(); c->tvecs.clear();
     c->rmats.push_back(m3_identity());
@@ -741,6 +748,7 @@ int kt_reset(kt_ctx* c)
         c->place->in_new.clear(); c->place->in_old.clear();
     }
     c->dense_poses.clear();                      // reset(): densePoseGraph.clear(), latestDensePoseId = 0 (.cpp:300-301)
+    if (c->mapvol && (r0 = mapvol_empty(c->mapvol.get(), c->stream))) return r0;
     c->trace_iters = 0; c->shifted_last = 0; c->cloud_count = 0;
     c->pf_valid = false; c->pf_built = false; c->frontend_ready = false; c->maps_on_stream = false;
     if (c->stream_copy) cudaStreamSynchronize(c->stream_copy);
@@ -1954,6 +1962,102 @@ int kt_save_map_ply(kt_ctx* c, const char* path, int which, int weld, kt_weld_re
     size_t nv = 0, nt = 0;
     int r = map_mesh(c, which, weld != 0, 0, 0, 0, 0, &v, &t, &nv, &nt, report, "kt_save_map_ply"); if (r) return r;
     return write_mesh_ply(path, std::vector<PlyPart>(1, PlyPart{v.data(), nv, t.data(), nt}), "kt_save_map_ply");
+}
+
+int kt_set_map_volume(kt_ctx* c, int enabled, size_t max_bricks)
+{
+    const char* who = "kt_set_map_volume";
+    if (!c) return KT_ERR_INVALID;
+    if (c->world > 1) { set_error("%s: a volume shared by %d GPUs has no map volume", who, c->world); return KT_ERR_INVALID; }
+    KT_CUDA(cudaSetDevice(c->cfg.device));
+    if (!enabled) {
+        if (c->mapvol) { KT_CUDA(cudaStreamSynchronize(c->stream)); c->mapvol.reset(); }
+        return KT_OK;
+    }
+    std::unique_ptr<MapVolume> m(new MapVolume());
+    int r = mapvol_init(m.get(), max_bricks, c->stream); if (r) return r;        // a refusal leaves the current store (or none) in place
+    KT_CUDA(cudaStreamSynchronize(c->stream));
+    c->mapvol = std::move(m);
+    return KT_OK;
+}
+
+static int map_volume_on(kt_ctx* c, const char* who)
+{
+    if (c->world > 1) { set_error("%s: a volume shared by %d GPUs has no map volume", who, c->world); return KT_ERR_INVALID; }
+    if (!c->mapvol) { set_error("%s: the map volume is off (kt_set_map_volume)", who); return KT_ERR_STATE; }
+    KT_CUDA(cudaSetDevice(c->cfg.device));
+    return KT_OK;
+}
+
+int kt_get_map_volume_info(kt_ctx* c, size_t* bricks, size_t* capacity, int* full)
+{
+    if (!c || !bricks || !capacity || !full) { set_error("kt_get_map_volume_info: bad argument"); return KT_ERR_INVALID; }
+    int r = map_volume_on(c, "kt_get_map_volume_info"); if (r) return r;
+    *capacity = c->mapvol->capacity;
+    return mapvol_info(c->mapvol.get(), bricks, full, c->stream);
+}
+
+int kt_get_map_volume_bricks(kt_ctx* c, uint64_t* keys, int16_t* tsdf, uint8_t* color, size_t max_bricks, size_t* n_bricks)
+{
+    if (!c || !n_bricks) { set_error("kt_get_map_volume_bricks: bad argument"); return KT_ERR_INVALID; }
+    int r = map_volume_on(c, "kt_get_map_volume_bricks"); if (r) return r;
+    return mapvol_bricks(c->mapvol.get(), (unsigned long long*)keys, tsdf, color, max_bricks, n_bricks, c->stream);
+}
+
+// The map mesh into host memory: up to the capacities (verts / tris may be null), or, with gv / gt, into host vectors of the full size
+static int global_mesh(kt_ctx* c, int weight_cull, kt_mesh_vertex* verts, size_t max_verts, uint32_t* tris, size_t max_tris,
+                       std::vector<kt_mesh_vertex>* gv, std::vector<uint32_t>* gt, size_t* n_verts, size_t* n_tris, kt_global_mesh_report* report,
+                       const char* who)
+{
+    kt_global_mesh_report R; std::memset(&R, 0, sizeof(R));
+    if (report) *report = R;
+    *n_verts = 0; *n_tris = 0;
+    int r = map_volume_on(c, who); if (r) return r;
+    cudaStream_t s = c->stream;
+    Allocations out(s);
+    kt_mesh_vertex* d_v = 0; uint32_t* d_t = 0;
+    const bool fetch = gv || verts || tris;
+    const MeshOutput sink = [&](size_t nv, size_t nt, void** v, uint32_t** t) -> int {
+        if (!fetch) return 1;
+        if (out.device(&d_v, nv, who) || out.device(&d_t, 3 * nt, who)) return KT_ERR_CUDA;
+        *v = d_v; *t = d_t;
+        return 0;
+    };
+    size_t nv = 0, nt = 0;
+    float3 vs = make_float3(c->size, c->size, c->size);
+    if ((r = mapvol_mesh(c->mapvol.get(), c->tsdf, c->color, c->cfg.vol, c->voxelWrap, vs, weight_cull, sink, &nv, &nt, &R, s))) return r;
+    if (gv) { gv->resize(nv); gt->resize(3 * nt); verts = gv->data(); tris = gt->data(); max_verts = nv; max_tris = nt; }
+    const size_t kv = verts ? std::min(nv, max_verts) : 0, kt = tris ? std::min(nt, max_tris) : 0;
+    if (kv || kt) {
+        cudaEvent_t ev[2];
+        for (int e = 0; e < 2; ++e) if (out.event(&ev[e], cudaEventDefault, who)) return KT_ERR_CUDA;
+        KT_CUDA(cudaEventRecord(ev[0], s));
+        if (kv) KT_CUDA(cudaMemcpyAsync(verts, d_v, kv * sizeof(kt_mesh_vertex), cudaMemcpyDeviceToHost, s));
+        if (kt) KT_CUDA(cudaMemcpyAsync(tris, d_t, kt * 3 * sizeof(uint32_t), cudaMemcpyDeviceToHost, s));
+        KT_CUDA(cudaEventRecord(ev[1], s));
+        KT_CUDA(cudaStreamSynchronize(s));
+        KT_CUDA(cudaEventElapsedTime(&R.download_ms, ev[0], ev[1]));
+        R.total_ms += R.download_ms;
+    }
+    *n_verts = nv; *n_tris = nt;
+    if (report) *report = R;
+    return KT_OK;
+}
+
+int kt_get_global_mesh(kt_ctx* c, int weight_cull, kt_mesh_vertex* verts, size_t max_verts, uint32_t* tris, size_t max_tris, size_t* n_verts,
+                       size_t* n_tris, kt_global_mesh_report* report)
+{
+    if (!c || !n_verts || !n_tris) { set_error("kt_get_global_mesh: bad argument"); return KT_ERR_INVALID; }
+    return global_mesh(c, weight_cull, verts, max_verts, tris, max_tris, 0, 0, n_verts, n_tris, report, "kt_get_global_mesh");
+}
+
+int kt_save_global_mesh_ply(kt_ctx* c, const char* path, int weight_cull, kt_global_mesh_report* report)
+{
+    if (!c || !path) { set_error("kt_save_global_mesh_ply: bad argument"); return KT_ERR_INVALID; }
+    std::vector<kt_mesh_vertex> v; std::vector<uint32_t> t;
+    size_t nv = 0, nt = 0;
+    int r = global_mesh(c, weight_cull, 0, 0, 0, 0, &v, &t, &nv, &nt, report, "kt_save_global_mesh_ply"); if (r) return r;
+    return write_mesh_ply(path, std::vector<PlyPart>(1, PlyPart{v.data(), nv, t.data(), nt}), "kt_save_global_mesh_ply");
 }
 
 int kt_get_slice_info(kt_ctx* c, int idx, kt_slice_info* info)

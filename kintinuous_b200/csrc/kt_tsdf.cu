@@ -393,7 +393,7 @@ int init_shared(const VolumeView& vv, int vol, cudaStream_t s)
     return fill_zero(vv.color[vv.rank], plane * (vol / vv.world) * 4, s);
 }
 
-int clear_volume_shared(int axis, int back, const VolumeView& vv, int vol, int current, int delta, cudaStream_t s)
+void clear_range(int axis, int back, int vol, int current, int delta, int* first, int* planes)
 {
     const int V = vol;
     const int n = delta - current;
@@ -405,8 +405,16 @@ int clear_volume_shared(int axis, int back, const VolumeView& vv, int vol, int c
         int reach = (an % 16 != 0) ? (an + 16 - an % 16) : an;
         if (count > reach) count = reach;
     }
-    if (count <= 0) return 0;
     if (count > V) count = V;
+    *first = p0; *planes = count > 0 ? count : 0;
+}
+
+int clear_volume_shared(int axis, int back, const VolumeView& vv, int vol, int current, int delta, cudaStream_t s)
+{
+    const int V = vol;
+    int p0, count;
+    clear_range(axis, back, vol, current, delta, &p0, &count);
+    if (count <= 0) return 0;
     int16_t* tsdf = vv.tsdf[vv.rank]; uint8_t* color = vv.color[vv.rank];
     if (axis == 0) {
         size_t total = (size_t)count * V * V;
