@@ -13,7 +13,8 @@
 //   * centroids accumulate in 64-bit fixed point (2^-32 m) with integer atomics: order-independent, hence deterministic run to run
 //     (PCL's float sums depend on std::sort's unspecified order inside a leaf); colours are integer sums, divided as PCL divides them;
 //   * the 20 nearest neighbours are found EXACTLY by one warp per point scanning the cube of +-r leaves around the point's leaf
-//     (r = 3, 4, ...; a point outside the cube is farther than r leaves, so the search stops as soon as the 20th candidate is nearer),
+//     (r = 3, 4, ...; a point outside the cube is farther than r leaves less a margin for float leaf assignment, derived from the grid's
+//     extent in leaf_grid, so the search stops as soon as the 20th candidate is nearer than that),
 //     candidates ranked by (squared distance, slot) -- the order the oracle uses -- in ONE pass (rank = number of smaller candidates);
 //   * the 3x3 covariance is taken about the query point (PCL's single-pass float sum of raw coordinates loses ~3 digits to
 //     cancellation for clouds metres away from the origin) and its smallest eigenpair comes from PCL's analytic eigen33 in FP64;
@@ -30,7 +31,8 @@ namespace {
 
 enum { SL_THREADS = 256, NRM_THREADS = 128, KNN_MAX = 32, CAND_CAP = 768, R_CAP = 10 };     // normals: 4 warps x 768 candidates x 8 B = 24 KB of shared memory
 
-struct SliceGrid { int min_b[3]; int div_b[3]; float inv_leaf; float leaf; unsigned long long cells; };
+// margin: in leaves, how much nearer than r a point outside the cube of +-r leaves may be (slice_normals_kernel's stop rule; leaf_grid)
+struct SliceGrid { int min_b[3]; int div_b[3]; float inv_leaf; float leaf; float margin; unsigned long long cells; };
 
 __device__ __forceinline__ unsigned int ord_f(float f) { unsigned int u = __float_as_uint(f); return (u & 0x80000000u) ? ~u : (u | 0x80000000u); }
 __host__ __device__ __forceinline__ float unord_f(unsigned int u) { u = (u & 0x80000000u) ? (u & 0x7fffffffu) : ~u;
@@ -328,8 +330,8 @@ slice_normals_kernel(kt_point_xyzrgbnormal* __restrict__ pts, const SliceAcc* __
                 }
                 __syncwarp();
                 const float dk = sd[take - 1];
-                // a point outside the cube of +-r leaves is farther than r leaves from the query along some axis
-                const float reach = ((float)r - 0.001f) * g.leaf;
+                // a point outside the cube of +-r leaves is farther than r - g.margin leaves from the query along some axis
+                const float reach = ((float)r - g.margin) * g.leaf;
                 if (covers || ((int)m >= kk && dk <= reach * reach)) { done = true; ncand = (unsigned int)take; }
                 __syncwarp();
             }
@@ -450,6 +452,14 @@ int leaf_grid(const kt_point_xyzrgb* in, size_t n, int weight_cull, float leaf, 
         const int max_b = (int)floorf(mx[a] * g.inv_leaf);
         g.div_b[a] = max_b - g.min_b[a] + 1;
     }
+    // The kNN stop rule's margin.  A leaf is floor(fl(x * inv_leaf)): with U = ulp(max |fl(x * inv_leaf)|) over the grid, each point's
+    // fl(x * inv_leaf) is within U / 2 of x * inv_leaf, and each float centroid within U of its leaf's mean (ulp(x) * inv_leaf <= 2 U),
+    // so a point whose leaf lies beyond the +-r cube of the query's leaf is farther than r - 3 U leaves of 1 / inv_leaf along that axis.
+    // 1 / inv_leaf and the float distance key differ from the leaf and the exact square by a few 2^-24 relative (< 1e-5 leaf at r = 10).
+    // margin = 0.001 + 4 U covers both; 1.1e-3 leaf for a slice a few metres from the origin, >= 0.032 leaf once x * inv_leaf passes 2^16.
+    float big = 0.f;
+    for (int a = 0; a < 3; ++a) big = fmaxf(big, fmaxf(fabsf(mn[a] * g.inv_leaf), fabsf(mx[a] * g.inv_leaf)));
+    g.margin = 0.001f + 4.0f * (nextafterf(big, INFINITY) - big);
     g.cells = (unsigned long long)g.div_b[0] * g.div_b[1] * g.div_b[2];
     const size_t words = (size_t)((g.cells + 31) / 32);
     if ((r = slice_ws_reserve(ws, words, kept))) return r;
