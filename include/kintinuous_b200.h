@@ -272,12 +272,27 @@ KT_API int kt_save_map_ply(kt_ctx* ctx, const char* path, int which, int weld, k
  *     kt_get_slice_mesh_keys).  Bricks are keyed (bz + 2^20) << 42 | (by + 2^20) << 21 | (bx + 2^20) (21 signed bits per axis, z most
  *     significant); voxel (x, y, z) of brick b is global voxel 8 b + (x, y, z), stored at x + 8 y + 64 z.
  *   - Capacity is all or nothing per cleared slab: when a slab's new bricks do not all fit, none is stored (bricks already stored are
- *     still updated), `full` is set and tracking carries on.  Three kernel launches per cleared slab on the tracker stream, no host synchronisation; frames without a shift launch
- *     nothing more.  Off by default.
+ *     still updated), `full` is set and tracking carries on.  Three kernel launches per cleared slab on the tracker stream (four with
+ *     restore, below), no host synchronisation; frames without a shift launch nothing more.  Off by default.
  * kt_set_map_volume(ctx, 1, max_bricks) allocates an empty store of max_bricks bricks (3 KB each plus 24 B of hash per brick) up front,
  * replacing any current one; KT_ERR_CUDA when the memory is refused, and then nothing else changes.  enabled = 0 frees it.  kt_reset
  * empties it.  KT_ERR_INVALID for a volume shared by several GPUs (world > 1); the calls below return KT_ERR_STATE while it is off. */
 KT_API int kt_set_map_volume(kt_ctx* ctx, int enabled, size_t max_bricks);
+/* Restore: the store flows back into the moving volume, so that a camera returning to mapped space tracks against the surface it fused
+ * there and keeps averaging into it (instead of a blank volume, whose few new frames would later overwrite the stored surface).
+ *   - A shift clears storage planes [first, first + planes) along an axis (the store's set: Q13's round_up16 reach on x and Q12's ZMinus
+ *     slab included).  Once the clear has run, with wrap' the signed voxel wrap after this axis moves, every voxel of those planes whose
+ *     global voxel (logical voxel + wrap') lies in a stored brick with W != 0 there takes the stored tsdf and colour words, bit for bit;
+ *     every other voxel stays cleared.  Per axis, in x, y, z order: store -> clear -> restore, one more launch, no host synchronisation.
+ *     A later axis of the same frame stores the voxels this one restored, which changes nothing; kt_get_global_mesh's field is unchanged.
+ *   - The planes a clear reaches beyond those that leave the volume keep their global voxels, so their surface bricks come back in the
+ *     same frame: with restore on, the volume (and so tracking) can differ from restore off, and from the reference, at the first shift
+ *     that clears surface, even without a revisit.  Only bricks holding a surface are stored, so free space outside them is not
+ *     restored: a ray through it sees cleared voxels, as after any clear.
+ * Off by default; it belongs to the context and applies to the clears that follow (never to planes that entered before).  kt_reset and a
+ * replacing kt_set_map_volume(ctx, 1, n) keep it, kt_set_map_volume(ctx, 0, ...) turns it off.  It is a host flag read at the next
+ * shift, so it may change between any two frames.  KT_ERR_STATE while the map volume is off, KT_ERR_INVALID for world > 1. */
+KT_API int kt_set_map_volume_restore(kt_ctx* ctx, int enabled);
 KT_API int kt_get_map_volume_info(kt_ctx* ctx, size_t* bricks, size_t* capacity, int* full);
 /* The stored bricks sorted by key: keys, tsdf (512 int16 per brick) and colour (512 x 4 uint8: b, g, r, weight per voxel, the volume's
  * layout); any output may be NULL.  *n_bricks = the count; KT_ERR_CAPACITY (nothing copied) when it exceeds max_bricks. */

@@ -353,6 +353,10 @@ class Tracker:
         """The map volume (kt_set_map_volume): a sparse global TSDF of every voxel a shift clears, in 8^3 bricks; 0 frees it."""
         _check(self.lib.kt_set_map_volume(self.h, int(enabled), C.c_size_t(max_bricks)))
 
+    def set_map_volume_restore(self, enabled=True):
+        """Refill the planes each shift clears from the map volume (kt_set_map_volume_restore); needs the map volume on."""
+        _check(self.lib.kt_set_map_volume_restore(self.h, int(enabled)))
+
     def map_volume_info(self):
         """(bricks stored, capacity, full) of the map volume."""
         b = C.c_size_t(0); cap = C.c_size_t(0); full = C.c_int(0)

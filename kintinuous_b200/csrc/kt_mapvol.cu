@@ -13,6 +13,10 @@
 //   * capacity is all or nothing per clear: mark (insert the new keys) -> roll back (when they do not all fit, every key inserted by
 //     this clear is removed again; a no-op launch otherwise) -> write (the values; its first thread commits or restores the count and
 //     sets `full`).  Three launches per cleared slab on the tracker stream, no host synchronisation, nothing on frames without a shift.
+//   * restore (kt_set_map_volume_restore, off by default): once the clear has run, one more launch gives every voxel of the same planes
+//     the stored value of its global voxel under the wrap after the shift, where a stored brick holds it with W != 0.  Keys come from
+//     coordinates alone (one lookup per distinct key of a warp), so the volume is only written.  The planes Q13 / Q12 clear beyond those
+//     that leave keep their global voxels, so their surface bricks come back in the same frame; free space outside stored bricks does not.
 //   * export: the live volume's surface bricks and the store's, sorted and made unique with CUB, are merged into one brick set of S
 //     (a live voxel with W != 0 wins) -> marching cubes over the brick set: per brick an 11^3 tile of validity and raw values in shared
 //     memory (the brick, one voxel below, two above: classification needs the 3x3x3 neighbourhood, the normal of an edge's far end one
@@ -188,6 +192,35 @@ mapvol_write_kernel(const ClearRegion r, const StoreView m)
         if (key == EMPTY_KEY || b == NO_BRICK) continue;
         const size_t at = (size_t)b * MAPVOL_BRICK_VOXELS + local_of(gx, gy, gz);
         m.tsdf[at] = raw; m.color[at] = col;
+    }
+}
+
+// restore, after the clear: every voxel of the region (r.wrap = the wrap after the shift) whose global voxel has a stored value with
+// W != 0 takes that value.  Keys come from coordinates alone, so the volume is only written; no atomics.
+__global__ void __launch_bounds__(STORE_THREADS)
+mapvol_restore_kernel(const ClearRegion r, const StoreView m, int16_t* tsdf, uchar4* color)
+{
+    const unsigned int lane = threadIdx.x & 31;
+    for (long long base = (long long)blockIdx.x * blockDim.x; base < r.total; base += (long long)gridDim.x * blockDim.x) {
+        const long long i = base + threadIdx.x;
+        int sx = 0, sy = 0, sz = 0, gx = 0, gy = 0, gz = 0;
+        unsigned long long key = EMPTY_KEY;
+        if (i < r.total) {
+            region_voxel(r, i, sx, sy, sz);
+            gx = global_of(sx, r.wbase.x, r.wrap.x, r.V); gy = global_of(sy, r.wbase.y, r.wrap.y, r.V); gz = global_of(sz, r.wbase.z, r.wrap.z, r.V);
+            if (brick_ok(gx >> 3) && brick_ok(gy >> 3) && brick_ok(gz >> 3)) key = key_of(gx >> 3, gy >> 3, gz >> 3);
+        }
+        const unsigned int same = __match_any_sync(0xffffffffu, key);
+        const int leader = __ffs(same) - 1;
+        unsigned int b = NO_BRICK;
+        if (key != EMPTY_KEY && (int)lane == leader) b = lookup(m.slot_key, m.slot_val, m.slots, key);
+        b = __shfl_sync(0xffffffffu, b, leader);
+        if (b == NO_BRICK) continue;
+        const size_t at = (size_t)b * MAPVOL_BRICK_VOXELS + local_of(gx, gy, gz);
+        const uchar4 col = m.color[at];
+        if (col.w == 0) continue;
+        const size_t a = ((size_t)sz * r.V + sy) * r.V + sx;
+        tsdf[a] = m.tsdf[at]; color[a] = col;
     }
 }
 
@@ -470,6 +503,18 @@ int mapvol_store(MapVolume* m, const int16_t* tsdf, const uint8_t* color, int vo
     mapvol_rollback_kernel<<<grid_for(m->slots), STORE_THREADS, 0, s>>>(v);
     KT_LAUNCH_CHECK();
     mapvol_write_kernel<<<grid, STORE_THREADS, 0, s>>>(r, v);
+    KT_LAUNCH_CHECK();
+    return 0;
+}
+
+int mapvol_restore(MapVolume* m, int16_t* tsdf, uint8_t* color, int vol, const int* wrap_after, int axis, int first, int planes, cudaStream_t s)
+{
+    if (planes <= 0) return 0;
+    ClearRegion r;
+    r.tsdf = nullptr; r.color = nullptr; r.V = vol; r.axis = axis; r.first = first; r.planes = planes;
+    r.wrap = make_int3(wrap_after[0], wrap_after[1], wrap_after[2]); r.wbase = wrap_mod3(r.wrap, vol);
+    r.total = (long long)planes * vol * vol;
+    mapvol_restore_kernel<<<grid_for((size_t)r.total), STORE_THREADS, 0, s>>>(r, view(m), tsdf, (uchar4*)color);
     KT_LAUNCH_CHECK();
     return 0;
 }

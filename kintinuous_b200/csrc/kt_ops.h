@@ -288,6 +288,9 @@ int mapvol_empty(MapVolume* m, cudaStream_t s);
 // before a clear of storage planes [first, first + planes) along axis (clear_range): keep their voxels; wrap = the signed voxel wrap.
 // Three launches, asynchronous.
 int mapvol_store(MapVolume* m, const int16_t* tsdf, const uint8_t* color, int vol, const int* wrap, int axis, int first, int planes, cudaStream_t s);
+// after that clear: every voxel of the same planes whose global voxel under wrap_after (the signed wrap once this axis has moved) has a
+// stored value with W != 0 takes it; the others stay cleared.  One launch, asynchronous; the volume is written, never read.
+int mapvol_restore(MapVolume* m, int16_t* tsdf, uint8_t* color, int vol, const int* wrap_after, int axis, int first, int planes, cudaStream_t s);
 int mapvol_info(MapVolume* m, size_t* bricks, int* full, cudaStream_t s);          // synchronises s
 // the store sorted by key into host arrays (any may be null); *n = bricks; KT_ERR_CAPACITY beyond max.  Synchronises s.
 int mapvol_bricks(MapVolume* m, unsigned long long* keys, int16_t* tsdf, uint8_t* color, size_t max, size_t* n, cudaStream_t s);

@@ -244,6 +244,7 @@ struct kt_ctx {
     DeviceBuffer<uint8_t> view;                                         // GUI taps: shaded image, colour image, model depth (allocated on first use)
     std::unique_ptr<PlaceStore> place;                                  // loop detection (null while it is off)
     std::unique_ptr<MapVolume> mapvol;                                  // the map volume (kt_mapvol.cu; null while it is off)
+    bool mapvol_restore = false;                                        // the map volume refills the planes a shift clears
     // what member destructors cannot do: wait for the streams, unmap the peers' arenas, close the pose log
     ~kt_ctx()
     {
@@ -647,12 +648,17 @@ int process_frame_device(kt_ctx* c, uint64_t utime, kt_pose* out)
             if ((r = fetch_cloud(c, vWrapCopy, lo, hi))) return r;
             if (c->slice_meshing && (r = mesh_box(c, vWrapCopy, lo, hi, true))) return r;
             if ((r = mg_barrier(c))) return r;                          // peers may still read my boundary plane for their extraction
+            int first = 0, planes = 0;
             if (c->mapvol) {                                            // keep what the clear is about to zero
-                int first, planes;
                 clear_range(axis, dir < 0 ? 1 : 0, V, c->voxelWrap[axis], c->voxelWrap[axis] + n, &first, &planes);
                 if ((r = mapvol_store(c->mapvol.get(), c->tsdf, c->color, V, c->voxelWrap, axis, first, planes, c->stream))) return r;
             }
             if ((r = clear_volume_shared(axis, dir < 0 ? 1 : 0, c->vv, V, c->voxelWrap[axis], c->voxelWrap[axis] + n, c->stream))) return r;
+            if (c->mapvol && c->mapvol_restore) {                       // give the cleared planes back what the store holds for them
+                int after[3] = {c->voxelWrap[0], c->voxelWrap[1], c->voxelWrap[2]};
+                after[axis] += n;
+                if ((r = mapvol_restore(c->mapvol.get(), c->tsdf, c->color, V, after, axis, first, planes, c->stream))) return r;
+            }
         }
         if (cycled) {                                                                    // mutexOutCloudBuffer (.cpp:1156-1208)
             int vt[3] = {0, 0, 0}; vt[axis] = n;
@@ -1972,6 +1978,7 @@ int kt_set_map_volume(kt_ctx* c, int enabled, size_t max_bricks)
     KT_CUDA(cudaSetDevice(c->cfg.device));
     if (!enabled) {
         if (c->mapvol) { KT_CUDA(cudaStreamSynchronize(c->stream)); c->mapvol.reset(); }
+        c->mapvol_restore = false;
         return KT_OK;
     }
     std::unique_ptr<MapVolume> m(new MapVolume());
@@ -1986,6 +1993,14 @@ static int map_volume_on(kt_ctx* c, const char* who)
     if (c->world > 1) { set_error("%s: a volume shared by %d GPUs has no map volume", who, c->world); return KT_ERR_INVALID; }
     if (!c->mapvol) { set_error("%s: the map volume is off (kt_set_map_volume)", who); return KT_ERR_STATE; }
     KT_CUDA(cudaSetDevice(c->cfg.device));
+    return KT_OK;
+}
+
+int kt_set_map_volume_restore(kt_ctx* c, int enabled)
+{
+    if (!c) return KT_ERR_INVALID;
+    int r = map_volume_on(c, "kt_set_map_volume_restore"); if (r) return r;
+    c->mapvol_restore = enabled != 0;                           // read by the next shift on the host: no device work here
     return KT_OK;
 }
 

@@ -1,8 +1,12 @@
 """What the map volume costs (kt_mapvol.cu), as one JSON line.
 
-  store: the synthetic stream (640x480, voxel shift 2) tracked at 512^3 and 1024^3 with the map volume off and on; the frame time is a
-         host clock around each frame, which ends in a synchronise.  Shift frames carry the store's three launches per cleared slab, so
-         the difference of their medians is what a shift costs; frames without a shift should not change.
+  store: the synthetic stream (640x480, voxel shift 2) tracked at 512^3 and 1024^3 with the map volume off, on, and on with restore;
+         the frame time is a host clock around each frame, which ends in a synchronise.  Shift frames carry the store's three launches
+         per cleared slab (four with restore), so the difference of their medians is what a shift costs; frames without a shift should
+         not change.
+  drift: a noisy out-and-back stream (640x480 into 128^3 and 256^3 over 3 m, voxel shift 2, 0.025 m per frame along +-x, +-y, +-z) tracked with
+         the map volume on, restore off and on: the translation error against the rendered ground truth per frame, its maximum, and
+         at each return to the start.
   export: kt_op_mesh_bricks over every brick with a surface voxel of a sphere in a 1024^3 grid, CUDA events around the call.
 
 Usage: python tools/map_volume_bench.py [--frames 120] [--repeat 5]
@@ -28,13 +32,14 @@ def _gpu():
         return "unknown"
 
 
-def tracker_cost(kb, vol, frames, store):
-    """Frame times (ms, host clock around each synchronous frame) and launches of the shifting stream, store on or off."""
+def tracker_cost(kb, vol, frames, store, restore=False):
+    """Frame times (ms, host clock around each synchronous frame) and launches of the shifting stream, store on or off, restore on or off."""
     from kintinuous_b200 import synth
     rows, cols = 480, 640
     trk = kb.Tracker(kb.Config.default(rows=rows, cols=cols, vol=vol, odometry=0, voxel_shift=2))
     if store:
         trk.set_map_volume(True, 1 << 20)
+        trk.set_map_volume_restore(restore)
     seq = [synth.render(k, cols, rows) for k in range(frames)]
     times, shift_times, launches = [], [], 0
     for k, (d, c) in enumerate(seq):
@@ -51,6 +56,31 @@ def tracker_cost(kb, vol, frames, store):
     return {"frame_ms_median": float(np.median(times)), "shift_frame_ms_median": float(np.median(shift_times)) if shift_times else None,
             "shift_frames": len(shift_times), "launches": launches, "bricks": int(info[0]), "brick_mb": info[0] * 3072 / 2 ** 20,
             "export": gm}
+
+
+def drift(kb, restore, vol, leg=20, step=0.025):
+    """Per-frame translation error (m) of the noisy out-and-back stream against its ground truth, restore off or on.  The tracked
+    position is the volume-relative translation plus the voxel wrap."""
+    from kintinuous_b200 import synth
+    rows, cols = 480, 640
+    trk = kb.Tracker(kb.Config.default(rows=rows, cols=cols, vol=vol, volume_size=3.0, odometry=0, voxel_shift=2))
+    trk.set_map_volume(True, 1 << 16)
+    trk.set_map_volume_restore(restore)
+    steps, traj = np.zeros(3, np.int64), [np.zeros(3, np.int64)]
+    for axis, sgn in ((0, 1), (0, -1), (1, 1), (1, -1), (2, 1), (2, -1)):
+        for _ in range(leg):
+            steps = steps.copy(); steps[axis] += sgn
+            traj.append(steps)
+    err, p0 = [], None
+    for k, s in enumerate(traj):
+        d, c = synth.render_at(np.eye(3), s * step, cols, rows, noise=True, noise_seed=k)
+        p = trk.process_frame(d, c, k)
+        pos = np.array(p.t, np.float64) + np.array(p.voxel_wrap, np.float64) * trk.voxel_size
+        p0 = pos if p0 is None else p0
+        err.append(float(np.linalg.norm((pos - p0) - s * step)))
+    trk.close()
+    home = [k for k in range(1, len(traj)) if not traj[k].any()]
+    return {"frames": len(traj), "err_m": [round(e, 6) for e in err], "err_max_m": max(err), "err_at_start_m": {str(k): err[k] for k in home}}
 
 
 def export_cost(kb, torch, repeat):
@@ -93,7 +123,10 @@ def main():
         raise SystemExit("map_volume_bench: no CUDA device")
     out = {"gpu": _gpu()}
     for vol in (512, 1024):
-        out[f"tracker_{vol}"] = {"off": tracker_cost(kb, vol, a.frames, False), "on": tracker_cost(kb, vol, a.frames, True)}
+        out[f"tracker_{vol}"] = {"off": tracker_cost(kb, vol, a.frames, False), "on": tracker_cost(kb, vol, a.frames, True),
+                                 "on_restore": tracker_cost(kb, vol, a.frames, True, True)}
+    for vol in (128, 256):
+        out[f"drift_out_and_back_{vol}"] = {"restore_off": drift(kb, False, vol), "restore_on": drift(kb, True, vol)}
     out["export_1024_sphere"] = export_cost(kb, torch, a.repeat)
     print(json.dumps(out))
 
