@@ -140,8 +140,9 @@ int reduce_grid_for(int n_items);
 int init_volume(int16_t* tsdf, uint8_t* color, int vol, cudaStream_t s);                  // whole volume
 int init_shared(const VolumeView& vv, int vol, cudaStream_t s);       // this rank's TSDF replica and colour planes
 int clear_volume(int axis, int back, int16_t* tsdf, uint8_t* color, int vol, int current_wrap, int delta_wrap, cudaStream_t s);
-// shared volume: the TSDF planes of the local replica and the colour planes this rank owns
-int clear_volume_shared(int axis, int back, const VolumeView& vv, int vol, int current_wrap, int delta_wrap, cudaStream_t s);
+// shared volume: zero the storage planes [first, first + planes) (mod vol) along `axis` that clear_range gives, in the local TSDF
+// replica and the colour planes this rank owns
+int clear_volume_shared(int axis, const VolumeView& vv, int vol, int first, int planes, cudaStream_t s);
 // the storage planes [first, first + planes) (mod vol) along `axis` that clear_volume zeroes (SURVEY.md Q13: an x clear reaches round_up_16)
 void clear_range(int axis, int back, int vol, int current_wrap, int delta_wrap, int* first, int* planes);
 int scale_depth(const uint16_t* depth, float* scaled, int rows, int cols, const Intr& k, bool angle_color, cudaStream_t s);

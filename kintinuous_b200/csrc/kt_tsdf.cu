@@ -383,7 +383,9 @@ int init_volume(int16_t* tsdf, uint8_t* color, int vol, cudaStream_t s)
 //   which drops the last plane exactly when |n| is a multiple of 16.
 int clear_volume(int axis, int back, int16_t* tsdf, uint8_t* color, int vol, int current, int delta, cudaStream_t s)
 {
-    return clear_volume_shared(axis, back, single_volume(tsdf, color, vol), vol, current, delta, s);
+    int first, planes;
+    clear_range(axis, back, vol, current, delta, &first, &planes);
+    return clear_volume_shared(axis, single_volume(tsdf, color, vol), vol, first, planes, s);
 }
 
 int init_shared(const VolumeView& vv, int vol, cudaStream_t s)
@@ -409,21 +411,19 @@ void clear_range(int axis, int back, int vol, int current, int delta, int* first
     *first = p0; *planes = count > 0 ? count : 0;
 }
 
-int clear_volume_shared(int axis, int back, const VolumeView& vv, int vol, int current, int delta, cudaStream_t s)
+int clear_volume_shared(int axis, const VolumeView& vv, int vol, int first, int planes, cudaStream_t s)
 {
     const int V = vol;
-    int p0, count;
-    clear_range(axis, back, vol, current, delta, &p0, &count);
-    if (count <= 0) return 0;
+    if (planes <= 0) return 0;
     int16_t* tsdf = vv.tsdf[vv.rank]; uint8_t* color = vv.color[vv.rank];
     if (axis == 0) {
-        size_t total = (size_t)count * V * V;
+        size_t total = (size_t)planes * V * V;
         int grid = (int)((total + 255) / 256 < (size_t)device_info().sm_count * 16 ? (total + 255) / 256 : (size_t)device_info().sm_count * 16);
-        clear_planes_x_kernel<<<grid, 256, 0, s>>>(tsdf, (uchar4*)color, V, p0, count, vv);
+        clear_planes_x_kernel<<<grid, 256, 0, s>>>(tsdf, (uchar4*)color, V, first, planes, vv);
     } else {
-        size_t total = (size_t)count * V * (V / 8);
+        size_t total = (size_t)planes * V * (V / 8);
         int grid = (int)((total + 255) / 256 < (size_t)device_info().sm_count * 16 ? (total + 255) / 256 : (size_t)device_info().sm_count * 16);
-        clear_planes_yz_kernel<<<grid, 256, 0, s>>>(tsdf, color, V, axis, p0, count, vv);
+        clear_planes_yz_kernel<<<grid, 256, 0, s>>>(tsdf, color, V, axis, first, planes, vv);
     }
     KT_LAUNCH_CHECK();
     return 0;
