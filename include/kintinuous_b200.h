@@ -396,7 +396,7 @@ typedef struct kt_place_result {
     float inlier_ratio;
     double fitness;                      /* -1 when not reached */
     int stage;                           /* kt_place_stage */
-    kt_loop_constraint constraint;       /* stage KT_PLACE_LOOP: time1 = time, time2 = candidate_time */
+    kt_loop_constraint constraint;       /* stages KT_PLACE_FITNESS and KT_PLACE_LOOP: constraint[] = the pose the fitness was measured at; KT_PLACE_LOOP: time1 = time, time2 = candidate_time, inliers */
     int closed;                          /* close = 1 and kt_close_loop accepted it */
     kt_loop_report report;               /* kt_close_loop's report (close = 1) */
 } kt_place_result;
@@ -621,6 +621,11 @@ KT_API int kt_op_pgo_optimise(const double* poses_dev, int n_nodes, const kt_pgo
  * position), kp 6 floats each (x, y, size, angle in radians, response, laplacian sign), desc 64 floats each; *n_out (host). */
 KT_API int kt_op_surf(const uint8_t* rgb_dev, int rows, int cols, float hessian_threshold, int max_features, float* kp_dev, float* desc_dev,
                       int* n_out, void* stream);
+/* kt_op_keypoints_3d -- Surf3DTools::calculate3dPointsSURF's lookup (Surf3DTools.h:82, :142-160), what kt_detect_loops runs on every
+ * keyframe's keypoints: kp n x 6 floats (kt_op_surf's layout, x and y used), depth rows*cols u16 mm, both device; xyz n x 3 floats
+ * (device) in the depth camera, NaN for a keypoint without a point (not within +-0.5 px of a pixel, strict, depth 0, or z >= 10 m). */
+KT_API int kt_op_keypoints_3d(const float* kp_dev, int n, const uint16_t* depth_dev, int rows, int cols, const float* intr4, float* xyz_dev,
+                              void* stream);
 /* kt_op_match_ratio -- the ratio test of Surf3DTools::surfMatch3D (Surf3DTools.h:105-140) with an exact 2-NN in place of FLANN, and the
  * retrieval kt_detect_loops runs with it: the database is n_seg segments (keyframes) of `stride` rows of 64 floats, of which the first
  * seg_counts[g] are valid (host array; NULL: all).  For each valid row the two nearest of n_query query descriptors (squared distances),

@@ -852,6 +852,14 @@ class _Ops:
         n = n.value
         return kp[:6 * n].cpu().numpy().reshape(n, 6), desc[:64 * n].cpu().numpy().reshape(n, 64)
 
+    def keypoints_3d(self, kp, depth, rows, cols, intr):
+        """kt_op_keypoints_3d on device keypoints kp [n, 6] and a device depth image: host float32 [n, 3], NaN rows without a point."""
+        import torch
+        n = int(kp.shape[0])
+        xyz = torch.empty(max(n, 1) * 3, dtype=torch.float32, device="cuda")
+        _check(self._l().kt_op_keypoints_3d(_ptr(kp), n, _ptr(depth), rows, cols, _ptr(_f(intr)), _ptr(xyz), None))
+        return xyz[:3 * n].cpu().numpy().reshape(n, 3)
+
     def match_ratio(self, db, query, ratio=0.49, stride=None, seg_counts=None):
         """kt_op_match_ratio on device descriptors db [n_seg * stride, 64] (stride None: one segment of all rows), query [m, 64]; seg_counts:
         valid rows per segment (None: all).  Returns host arrays (best, d1, d2, pass, passes per segment)."""

@@ -430,6 +430,19 @@ int kt_op_surf(const uint8_t* rgb, int rows, int cols, float thr, int max_featur
     return KT_OK;
 }
 
+int kt_op_keypoints_3d(const float* kp, int n, const uint16_t* depth, int rows, int cols, const float* k4, float* xyz, void* s)
+{
+    if (!kp || !depth || !k4 || !xyz || n < 0 || rows <= 0 || cols <= 0) { set_error("kt_op_keypoints_3d: bad argument"); return KT_ERR_INVALID; }
+    if (n == 0) return KT_OK;
+    KT_OPS_LOCK();
+    int* n_dev = 0; int r;
+    if ((r = place_ints(1, &n_dev))) return r;
+    KT_CUDA(cudaMemcpyAsync(n_dev, &n, sizeof(int), cudaMemcpyHostToDevice, st(s)));
+    if ((r = keypoints_3d(kp, n_dev, n, depth, rows, cols, intr4(k4), xyz, st(s)))) return r;
+    KT_CUDA(cudaStreamSynchronize(st(s)));
+    return KT_OK;
+}
+
 int kt_op_match_ratio(const float* db, int n_seg, int stride, const int* seg_counts, const float* q, int n_query, float ratio, int* best, float* d1,
                       float* d2, uint8_t* pass, int* seg_passes, void* s)
 {

@@ -161,7 +161,7 @@ __global__ void surf_extrema_kernel(const int* __restrict__ I, const SurfGeom g,
         // offset = -H^-1 g (Cramer)
         const double ox = -(dx * (hyy * hss - hys * hys) - hxy * (dy * hss - hys * ds) + hxs * (dy * hys - hyy * ds)) / det;
         const double oy = -(hxx * (dy * hss - ds * hys) - dx * (hxy * hss - hys * hxs) + hxs * (hxy * ds - dy * hxs)) / det;
-        const double os = -(hxx * (hyy * ds - hys * dy) - hxy * (hxy * ds - hys * dx) + dx * (hxy * hys - hyy * hxs)) / det;
+        const double os = -(hxx * (hyy * ds - hys * dy) - hxy * (hxy * ds - hxs * dy) + dx * (hxy * hys - hyy * hxs)) / det;
         if (fabs(ox) > 1.0 || fabs(oy) > 1.0 || fabs(os) > 1.0) continue;
         int lap;
         surf_det(I, g.cols + 1, surf_size(o, l), j << o, i << o, &lap);

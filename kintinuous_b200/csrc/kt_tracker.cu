@@ -1629,6 +1629,7 @@ int place_process(kt_ctx* c, int q, kt_place_result* res)
     size_t ns = 0, nd = 0;
     if ((r = cloud_fitness(ps->cloud[0], P, ps->cloud[1], P, 2.5f * c->voxel, T12, &ps->ws[0], &ps->ws[1], ps->cent[0], ps->cent[1], P, ps->d2fit, &res->fitness, &ns, &nd, s))) return r;
     res->stage = KT_PLACE_FITNESS;
+    for (int k = 0; k < 16; ++k) res->constraint.constraint[k] = C[k];      // the pose the fitness was measured at, loop or not
     if (!(res->fitness >= 0.0 && res->fitness < 0.01)) return 0;
     // the loop: inliers back-projected at their truncated pixels (DepthCamera::projectInlierMatches)
     std::vector<uint16_t> hd_new(P), hd_old(P);
@@ -1640,7 +1641,6 @@ int place_process(kt_ctx* c, int q, kt_place_result* res)
     place_project_inliers(kpn.data(), kpo.data(), inl.data(), m, hd_new.data(), hd_old.data(), ps->rows, ps->cols, intr, a1, a2);
     res->stage = KT_PLACE_LOOP;
     res->constraint.time1 = res->time; res->constraint.time2 = res->candidate_time;
-    for (int k = 0; k < 16; ++k) res->constraint.constraint[k] = C[k];
     res->constraint.n_inliers = a1.size() / 3;
     res->constraint.inliers1 = a1.empty() ? 0 : a1.data(); res->constraint.inliers2 = a2.empty() ? 0 : a2.data();
     return 0;

@@ -7,11 +7,14 @@ conversion and the PnP pose; scipy's cKDTree pins the fitness.
 """
 from __future__ import annotations
 
+import math
+
 import numpy as np
 
 OCTAVES, LAYERS = 4, 4
 HESSIAN = 400.0
 RATIO = 0.49
+U32 = 2.0 ** -24                            # float32 unit roundoff
 
 
 def grey(rgb):
@@ -129,8 +132,21 @@ def _haar(I, px, py, hs, rows, cols):
 _DISC = [(i, j) for j in range(-6, 7) for i in range(-6, 7) if i * i + j * j < 36]
 
 
-def describe(I, x, y, size, rows, cols):
-    """(angle in radians, 64-d unit descriptor) of one keypoint, as kt_surf.cu's surf_describe_kernel."""
+def _to_half(p):
+    """FP64 distance of positions p from the nearest rounding boundary of rint (k + 0.5)."""
+    return np.abs(p - (np.floor(p) + 0.5))
+
+
+def describe(I, x, y, size, rows, cols, margins=False):
+    """(angle in radians, 64-d unit descriptor) of one keypoint, as kt_surf.cu's surf_describe_kernel.  margins: also a dict of how far
+    the decisions float32 can flip lie from their edges --
+      ori         the best 60 degree window's squared length minus the runner-up's (the best window with other members: windows with
+                  the same members have the same sum on both sides), relative to the best; ori_bound: what float32 window sums can move it;
+      ori_edge    degrees between a sample of the best window and the window's edge (samples on an axis, exact on both sides, excluded);
+      sample      px between the FP64 position of any orientation or descriptor sample and a rint boundary (k + 0.5), the minimum;
+      sample_slack  the same minus each position's float32 rounding bound (<= 0: a sample may round to the other pixel);
+      sample_turn   the least change of the angle (radians) that moves a descriptor sample, float32 rounding included, across a boundary:
+                  a device angle closer than that to the oracle's samples the same pixels."""
     x32, y32 = np.float32(x), np.float32(y)
     sigma = np.float32(1.2) * np.float32(size) / np.float32(9.0)
     ij = np.array(_DISC)
@@ -140,15 +156,18 @@ def describe(I, x, y, size, rows, cols):
     dx, dy, ok = _haar(I, px, py, hs_o, rows, cols)
     w = np.exp(-(ij[:, 0] ** 2 + ij[:, 1] ** 2) / (2.0 * 2.5 * 2.5))
     dx, dy = dx * w, dy * w
+    dx_o, dy_o = dx, dy
     ang = np.degrees(np.arctan2(dy, dx)); ang = np.where(ang < 0, ang + 360.0, ang)
     use = ~((dx == 0) & (dy == 0))
-    best, bsx, bsy = -1.0, 0.0, 0.0
+    best, bsx, bsy, kb = -1.0, 0.0, 0.0, 0
+    wins = np.zeros(72)
     for k in range(72):
         d = np.abs(ang - 5.0 * k)
         m = use & ((d < 30.0) | (d > 330.0))
-        sx, sy = dx[m].sum(), dy[m].sum()
+        sx, sy = math.fsum(dx[m]), math.fsum(dy[m])           # correctly rounded: the same sum in any order
+        wins[k] = sx * sx + sy * sy
         if sx * sx + sy * sy > best:
-            best, bsx, bsy = sx * sx + sy * sy, sx, sy
+            best, bsx, bsy, kb = sx * sx + sy * sy, sx, sy, k
     th = float(np.arctan2(bsy, bsx))
     co, si = np.float32(np.cos(th)), np.float32(np.sin(th))
     u, v = np.meshgrid(np.arange(20), np.arange(20))
@@ -165,19 +184,51 @@ def describe(I, x, y, size, rows, cols):
             bx = rx[cv * 5:cv * 5 + 5, cu * 5:cu * 5 + 5]; by = ry[cv * 5:cv * 5 + 5, cu * 5:cu * 5 + 5]
             desc[(cv * 4 + cu) * 4:(cv * 4 + cu) * 4 + 4] = [bx.sum(), by.sum(), np.abs(bx).sum(), np.abs(by).sum()]
     n = np.linalg.norm(desc)
-    return th, desc / n if n > 0 else desc
+    desc = desc / n if n > 0 else desc
+    if not margins:
+        return th, desc
+    # windows whose member set equals the best's have its sum on both sides: the runner-up is the best window with other members
+    mem = [use & ((np.abs(ang - 5.0 * k) < 30.0) | (np.abs(ang - 5.0 * k) > 330.0)) for k in range(72)]
+    other = [wins[k] for k in range(72) if not np.array_equal(mem[k], mem[kb])]
+    ori = (best - max(other)) / best if best > 0 and other else (0.0 if best <= 0 else 1.0)
+    # float32 sums of <= 109 terms: |d sx| <= 110 u sum |dx|, so s^2 moves by at most 2 (110 u) (sum|dx| + sum|dy|) / |s| relative
+    mag = np.abs(dx_o[mem[kb]]).sum() + np.abs(dy_o[mem[kb]]).sum()
+    rel = 110 * U32 * mag / np.sqrt(best) if best > 0 else np.inf
+    e = np.abs(ang - 5.0 * kb)
+    edge = np.minimum(np.abs(e - 30.0), np.abs(e - 330.0))
+    exact = (dx_o == 0) | (dy_o == 0)                           # an axis direction: 0, 90, 180, 270 degrees on both sides
+    ori_edge = float(edge[use & ~exact].min()) if (use & ~exact).any() else np.inf
+    sig = float(sigma); x64, y64 = float(x32), float(y32)
+    ox64, oy64 = ox.astype(np.float64), oy.astype(np.float64)
+    po = [x64 + ij[:, 0] * sig, y64 + ij[:, 1] * sig]
+    pd = [x64 + float(co) * ox64 - float(si) * oy64, y64 + float(si) * ox64 + float(co) * oy64]
+    # float32 evaluation of a position, with any contraction: <= 4 roundings of magnitude |x| + |o|
+    bo = [4 * U32 * (abs(x64) + np.abs(ij[:, 0]) * sig), 4 * U32 * (abs(y64) + np.abs(ij[:, 1]) * sig)]
+    arm = np.abs(ox64) + np.abs(oy64)
+    bd = [4 * U32 * (abs(x64) + arm), 4 * U32 * (abs(y64) + arm)]
+    sample = float(min(_to_half(p_).min() for p_ in po + pd))
+    slack = float(min((_to_half(p_) - b_).min() for p_, b_ in zip(po, bo)))
+    # a descriptor sample moves by at most arm |d theta| when the angle changes: the least turn that can move one across a boundary
+    turn = float(min(((_to_half(p_) - b_) / arm).min() for p_, b_ in zip(pd, bd)))
+    return th, desc, dict(ori=float(ori), ori_bound=float(2 * rel), ori_edge=ori_edge, sample=sample, sample_slack=min(slack, turn * arm.max()),
+                          sample_turn=turn)
 
 
-def surf(rgb, max_features=1000, threshold=HESSIAN):
-    """(kp [n, 6] = x, y, size, angle, response, laplacian; desc [n, 64]) in the device's order."""
+def surf(rgb, max_features=1000, threshold=HESSIAN, margins=False):
+    """(kp [n, 6] = x, y, size, angle, response, laplacian; desc [n, 64]) in the device's order.  margins: also a dict of arrays [n]
+    (describe's ori, ori_edge and sample per keypoint)."""
     rows, cols = rgb.shape[:2]
     cands, I = detect(rgb, threshold)
     cands = cands[:max_features]
     kp = np.zeros((len(cands), 6)); desc = np.zeros((len(cands), 64))
+    mg = {k: np.zeros(len(cands)) for k in ("ori", "ori_bound", "ori_edge", "sample", "sample_slack", "sample_turn")}
     for k, (_, x, y, size, resp, lap) in enumerate(cands):
-        th, d = describe(I, x, y, size, rows, cols)
-        kp[k] = [x, y, size, th, resp, lap]; desc[k] = d
-    return kp, desc
+        r = describe(I, x, y, size, rows, cols, margins)
+        kp[k] = [x, y, size, r[0], resp, lap]; desc[k] = r[1]
+        if margins:
+            for key in mg:
+                mg[key][k] = r[2][key]
+    return (kp, desc, mg) if margins else (kp, desc)
 
 
 # ---- matching, lookup, candidate selection (kt_place.hpp) ----
@@ -233,6 +284,42 @@ def lookup_3d(x, y, depth, intr):
         return None
     fx, fy, cx, cy = [np.float32(a) for a in intr]
     return np.array([z * (np.float32(u) - cx) / fx, z * (np.float32(v) - cy) / fy, z], np.float32)
+
+
+def keypoints_3d(kp, depth, intr):
+    """kt_place.cu keypoints_3d_kernel: [n, 3] float32, the rule of lookup_3d in the device's float32 order (z = d / 1000, then
+    (z (u - cx)) / fx with one rounding per operation); NaN rows where a keypoint has no point."""
+    kp = np.asarray(kp, np.float32).reshape(len(kp), -1)
+    rows, cols = depth.shape
+    f32 = np.float32
+    x, y = kp[:, 0].astype(f32), kp[:, 1].astype(f32)
+    u = np.floor(x + f32(0.5)).astype(np.int64); v = np.floor(y + f32(0.5)).astype(np.int64)
+    ok = (np.abs(u.astype(f32) - x) < f32(0.5)) & (np.abs(v.astype(f32) - y) < f32(0.5)) & (u >= 0) & (v >= 0) & (u < cols) & (v < rows)
+    d = np.where(ok, depth[np.clip(v, 0, rows - 1), np.clip(u, 0, cols - 1)], 0)
+    z = d.astype(f32) / f32(1000.0)
+    ok &= (d != 0) & (z < f32(10.0))
+    fx, fy, cx, cy = [f32(a) for a in intr]
+    out = np.stack([(z * (u.astype(f32) - cx)) / fx, (z * (v.astype(f32) - cy)) / fy, z], 1).astype(f32)
+    out[~ok] = np.nan
+    return out
+
+
+def project_inliers(kp_new, kp_old, inlier, depth_new, depth_old, intr):
+    """kt_place.hpp place_project_inliers: every inlier's keypoints back-projected at their TRUNCATED pixels, pairs where either
+    depth is 0 (or a pixel is outside) dropped.  Returns (in_new [k, 3], in_old [k, 3]) float32."""
+    rows, cols = depth_new.shape
+    a, b = [], []
+    ifx, ify = 1.0 / float(np.float32(intr[0])), 1.0 / float(np.float32(intr[1]))
+    cx, cy = float(np.float32(intr[2])), float(np.float32(intr[3]))
+    for i in np.flatnonzero(np.asarray(inlier)):
+        u1, v1 = int(np.float32(kp_new[i][0])), int(np.float32(kp_new[i][1])); u2, v2 = int(np.float32(kp_old[i][0])), int(np.float32(kp_old[i][1]))
+        if min(u1, v1, u2, v2) < 0 or u1 >= cols or u2 >= cols or v1 >= rows or v2 >= rows:
+            continue
+        z1 = float(np.float32(depth_new[v1, u1]) / np.float32(1000.0)); z2 = float(np.float32(depth_old[v2, u2]) / np.float32(1000.0))
+        if z1 == 0.0 or z2 == 0.0:
+            continue
+        a.append([z1 * (u1 - cx) * ifx, z1 * (v1 - cy) * ify, z1]); b.append([z2 * (u2 - cx) * ifx, z2 * (v2 - cy) * ify, z2])
+    return np.array(a, np.float32).reshape(-1, 3), np.array(b, np.float32).reshape(-1, 3)
 
 
 def is_keyframe(R_curr, R_last, g_curr, g_last, movement=0.15):
@@ -349,3 +436,71 @@ def fitness(src_depth, dst_depth, intr, leaf, T):
     S2 = S @ T[:3, :3].T + T[:3, 3]
     d, _ = cKDTree(D).query(S2, k=1)
     return float((d * d).mean()), len(S), len(D)
+
+
+# ---- the verification of one candidate (kt_tracker.cu place_process after retrieval) ----
+RATIO32 = float(np.float32(RATIO))          # the device compares d1 < 0.49f d2
+MIN_MATCHES, PNP_SEED = 40, 0x4B696E74756F7573
+ICP_ITERS = (10, 5, 4, 0)                   # the tracker's ICP schedule, finest level first (ICPOdometry.cpp:42-55)
+
+
+def dense_icp(maps_old, maps_new, R0, t0, intr, iterations=ICP_ITERS):
+    """The dense check's point-to-plane ICP in FP64: the model is the old keyframe's maps with the camera at the identity, the current
+    frame the new keyframe's maps moved by (R0, t0) (float32, as transform_maps_pyramid).  Levels coarse to fine, `iterations[l]`
+    Gauss-Newton steps each, the systems of odometry_oracle.icp_system at the current pose (Rprev = I, tprev = 0), x = A^-1 b,
+    resultRt <- [rodrigues(x[3:]) | x[:3]] resultRt, pose = resultRt^-1.  maps_*: per level (vmap, nmap) [3, rows, cols] float32.
+    Returns (dT 4x4, ambiguous pixels summed over every step)."""
+    from . import odometry_oracle as OO
+    R0 = np.asarray(R0, np.float32).astype(np.float64); t0 = np.asarray(t0, np.float32).astype(np.float64)
+    res = np.eye(4); amb = 0
+    for level in range(len(iterations) - 1, -1, -1):
+        if iterations[level] == 0:
+            continue
+        vo, no = (np.asarray(a, np.float32) for a in maps_old[level])
+        vn, nn = (np.asarray(a, np.float64).reshape(3, -1) for a in maps_new[level])
+        vn = (R0 @ vn + t0[:, None]).astype(np.float32).astype(np.float64); nn = (R0 @ nn).astype(np.float32).astype(np.float64)
+        kl, _ = OO.level_intrinsics(*[np.float32(a) for a in intr], level)
+        for _ in range(iterations[level]):
+            T = np.linalg.inv(res)
+            v = (T[:3, :3] @ vn + T[:3, 3:4]).reshape(vo.shape); n = (T[:3, :3] @ nn).reshape(vo.shape)
+            S = OO.icp_system(v, n, vo, no, np.eye(3), np.zeros(3), kl)
+            amb += S.extra["ambiguous"]
+            x = np.linalg.solve(S.A, S.b)
+            M = np.eye(4); M[:3, :3] = OO._rodrigues(x[3:]); M[:3, 3] = x[:3]
+            res = M @ res
+    return np.linalg.inv(res), amb
+
+
+def verify(depth_old, kp_old, desc_old, depth_new, kp_new, desc_new, intr, maps_old, maps_new, voxel, inlier_ratio=0.35,
+           iterations=ICP_ITERS, ratio=RATIO32):
+    """place_process after retrieval, for candidate (old) and query (new) keyframes: 3-D matching, PnP, the inlier-ratio gate, the dense
+    ICP check, C = inv(dT Tp), fitness at 2.5 voxels and the projected inliers.  Returns a dict with every stage's value, the stage
+    where the chain stops (matches / inliers / fitness / loop, kt_place_result's names) and each gate's margin: matches - 40,
+    inlier ratio - threshold, 0.01 - fitness."""
+    out = dict(stage="matches")
+    xo = keypoints_3d(kp_old, depth_old, intr); xn = keypoints_3d(kp_new, depth_new, intr)
+    oi, ni = match_3d(desc_old, desc_new, xo, xn, ratio)
+    m = len(oi)
+    out.update(old_idx=oi, new_idx=ni, matches=m, margin_matches=m - MIN_MATCHES)
+    if m < MIN_MATCHES:
+        return out
+    pn, po = xn[ni], xo[oi]
+    uv = np.asarray(kp_old, np.float32)[oi, :2]
+    Rp, tp, inl = pnp_ransac(pn, po, uv, intr)
+    r = np.float32(inl.sum()) / np.float32(m)
+    out.update(stage="inliers", R_pnp=Rp, t_pnp=tp, inliers=inl, n_inliers=int(inl.sum()), inlier_ratio=float(r),
+               margin_ratio=float(r) - float(np.float32(inlier_ratio)))
+    if not r > np.float32(inlier_ratio):
+        return out
+    Tp = np.eye(4); Tp[:3, :3] = Rp; Tp[:3, 3] = tp
+    dT, amb = dense_icp(maps_old, maps_new, Rp, tp, intr, iterations)
+    C = np.linalg.inv(dT @ Tp)
+    leaf = float(np.float32(2.5) * np.float32(voxel))
+    f, ns, nd = fitness(depth_old, depth_new, intr, leaf, C.astype(np.float32))          # the device moves the cloud by (float) C
+    out.update(stage="fitness", dT=dT, C=C, icp_ambiguous=amb, fitness=f, n_src=ns, n_dst=nd, margin_fitness=0.01 - f)
+    if not (f >= 0.0 and f < 0.01):
+        return out
+    kn = np.asarray(kp_new, np.float32)[ni, :2]; ko = uv
+    a, b = project_inliers(kn, ko, inl, depth_new, depth_old, intr)
+    out.update(stage="loop", inliers1=a, inliers2=b)
+    return out
